@@ -10,7 +10,9 @@ A "step" is one full optimisation step (forward + backward + gradient all-reduce
 batch of 256 pairs per GPU (weak scaling), random-init weights of the named architecture, dropout 0.1 as configured.
 Rank 0 prints ONE JSON line.  `value` = device-resident inputs, CUDA-event timed, max over ranks; `e2e` = the same
 step through `Trainer.step` fed from pinned HOST buffers (H2D copy of every batch and D2H read of every loss inside
-the timed region).  `roofline` is for the dominant kernel (the tcgen05 GEMM, which runs every conv and linear layer).
+the timed region).  `roofline` is for the dominant kernel (the wgmma GEMM, which runs every conv and linear layer).
+`--dump-outputs DIR` writes what the last timed step returned and left behind (its losses and a fixed, seeded sample of
+the updated parameters and of the gradients) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -85,13 +87,39 @@ class ClockSampler:
                 "reasons": reasons, "samples": len(rows), "samples_in_timed_region": len(inside)}
 
 
-def measured_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            p = json.load(f)
-        return p.get("bf16_tflops_sustained", 1412.4), p.get("hbm_gbs", 6590.9), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+def datasheet_peaks():
+    """Dense bf16 tensor rate and HBM3 bandwidth of the H100 SXM data sheet (700 W card); not reached in practice."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3)"
+
+
+def gpu_identity(index):
+    """Name and power limit of the GPU the numbers were measured on (they belong beside every absolute number)."""
+    ident = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30)
+        ident["power_limit_w"] = float(out.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        pass
+    return ident
+
+
+DUMP_SAMPLE = 1 << 20  # elements of the parameter / gradient arenas written by --dump-outputs (seeded, fixed indices)
+
+
+def dump_outputs(out_dir, trainer, loss):
+    """The last timed step's results as float32 .npy files: its losses, and the same seeded sample of positions of the
+    parameter arena (after the update) and of the gradient arena (what the step computed before the update)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arena = trainer.engine.arena
+    n = arena.params.numel()
+    idx = torch.randperm(n, generator=torch.Generator().manual_seed(1234))[:min(DUMP_SAMPLE, n)].sort().values
+    idx = idx.to(arena.params.device)
+    outs = {"loss": loss.float(), "params_sample": arena.params[idx], "grads_sample": arena.grads[idx],
+            "sample_index": idx.double()}
+    for name, t in outs.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------------- CPU / reference
@@ -247,6 +275,8 @@ def main_ours(args, rank, world, local):
     e1.record()
     barrier()
     clocks.mark_end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer, loss)
     ms = max_over_ranks(e0.elapsed_time(e1))
     launches = ops.launch_count - launches0
     clk = clocks.stop() if rank == 0 else None
@@ -301,7 +331,7 @@ def main_ours(args, rank, world, local):
     ms_e2e = max_over_ranks(t0.elapsed_time(t1))
     e2e_value = args.steps * B * world / (ms_e2e / 1e3)
 
-    # ---- roofline of the dominant kernel: CUDA events around every tcgen05 GEMM launch of 2 further steps
+    # ---- roofline of the dominant kernel: CUDA events around every GEMM launch of 2 further steps
     roof = None
     if rank == 0:
         ops.start_gemm_profile()
@@ -318,7 +348,7 @@ def main_ours(args, rank, world, local):
                 json.dump([dict(ms=p[0], flops=p[1], M=p[2], N=p[3], K=p[4], conv_mode=p[5], a_mn=p[6], b_mn=p[7],
                                 extra_bytes=p[8])
                            for p in prof[len(prof) // 2:]], f)
-        peak_tf, peak_bw, peak_src = measured_peaks()
+        peak_tf, peak_bw, peak_src = datasheet_peaks()
         half = prof[len(prof) // 2:]  # the launches of the second profiled step
         g_ms = sum(p[0] for p in prof) / 2
         g_fl = sum(p[1] for p in prof) / 2
@@ -326,7 +356,7 @@ def main_ours(args, rank, world, local):
         def min_bytes(ms, fl, M, N, K, mode, a_mn, b_mn, extra):
             # operands read once + output written once (im2col-free for the implicit convs: the activation is counted
             # once, not once per tap) + what the epilogue reads besides (residual tile, ReLU bit mask)
-            if mode in (1, 3, 5):
+            if mode in (1, 5):
                 return 2 * (M * K // (9 if mode != 5 else 16) + N * K) + 2 * M * N + extra
             if mode in (2, 6):
                 return 2 * (K * M + K * N // (9 if mode != 6 else 16)) + 4 * M * N + extra
@@ -336,22 +366,9 @@ def main_ours(args, rank, world, local):
 
         g_by = sum(min_bytes(*p) for p in half)
         t_min = sum(max(p[1] / (peak_tf * 1e12), min_bytes(*p) / (peak_bw * 1e9)) for p in half) * 1e3  # ms
-        # DRAM bytes cannot be counted without ncu: `traffic` is the per-launch average of the committed ncu capture of
-        # this same command (profiles/, newest round first); traffic_source says which capture and at which commit
-        traffic = traffic_src = None
-        tnames = sorted((n for n in os.listdir(os.path.join(ROOT, "profiles")) if n.endswith("_gemm_dram_traffic.json")),
-                        reverse=True)  # newest capture first (r02s_ > r02_ > r01_)
-        for tname in tnames:
-            tpath = os.path.join(ROOT, "profiles", tname)
-            if os.path.exists(tpath):
-                with open(tpath) as f:
-                    tj = json.load(f)
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), f"profiles/{tname} @ {tj.get('commit', 'round-1 kernel')}"
-                break
-        roof = {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 GEMM: all convs + linears)",
+        roof = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (wgmma GEMM: all convs + linears)",
                 "achieved": round(g_fl / (g_ms * 1e-3) / 1e12, 1), "peak": peak_tf, "unit": "TFLOP/s",
-                "frac": round(g_fl / (g_ms * 1e-3) / 1e12 / peak_tf, 4), "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": peak_src,
+                "frac": round(g_fl / (g_ms * 1e-3) / 1e12 / peak_tf, 4), "peak_source": peak_src,
                 "launches_per_step": len(prof) // 2, "gemm_ms_per_step": round(g_ms, 3),
                 "gemm_share_of_step": round(g_ms / prof_ms, 3),
                 "algorithmic_gflop_per_launch": round(g_fl / 1e9 / (len(prof) // 2), 2),
@@ -381,8 +398,8 @@ def main_ours(args, rank, world, local):
                 "config": {"workload": f"bicaptioning {name} full optimisation step, batch {B} per GPU",
                            "config_file": args.config, "global_batch": B * world, "seq_len": T,
                            "parallelism": f"dp{world}", "dropout": cfg.MODEL.TEXTUAL.DROPOUT,
-                           "l2_policy": "per-step working set (>= 150 MB of inputs, GBs of activations) exceeds the 126 MB L2"},
-                "loss": round(loss_val, 4), "clocks": clk,
+                           "l2_policy": "per-step working set (>= 150 MB of inputs, GBs of activations) exceeds the 50 MB L2"},
+                "gpu": gpu_identity(local), "loss": round(loss_val, 4), "clocks": clk,
                 "e2e": {"value": round(e2e_value, 1), "unit": "pairs/s", "h2d_bytes_per_step": h2d,
                         "d2h_bytes_per_step": 8, "ms_per_step": round(ms_e2e / args.steps, 3),
                         "api": "virtex_b200.trainer.Trainer.step on pinned host batches"},
@@ -412,6 +429,8 @@ def main():
     ap.add_argument("--skip-cpu", action="store_true")
     ap.add_argument("--skip-incumbent", action="store_true")
     ap.add_argument("--dump-gemm-profile", default="")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's losses and seeded parameter / gradient samples as DIR/<name>.npy")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))

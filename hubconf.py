@@ -1,7 +1,7 @@
 """torch.hub entry point: drop-in for the reference's hubconf.py:10-35 (`resnet50(pretrained=False, **kwargs)`).
 
 Returns a module with torchvision's ResNet-50 parameter names (so the reference's released backbone weights load with
-`load_state_dict`), whose forward runs the sm_100a backbone kernels and -- like current torchvision with
+`load_state_dict`), whose forward runs the sm_90a backbone kernels and -- like current torchvision with
 `avgpool = fc = Identity` -- returns the flattened (B, 2048*h*w) layer4 features.  No download: there is no network.
 """
 dependencies = ["torch"]

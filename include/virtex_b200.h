@@ -1,5 +1,5 @@
 /*
- * virtex_b200 -- C ABI of the B200-native (sm_100a) kernels behind the VirTex bicaptioning pretraining step.
+ * virtex_b200 -- C ABI of the H100-native (sm_90a) kernels behind the VirTex bicaptioning pretraining step.
  *
  * The reference (kdexd/virtex) has no FFI of its own: its hot path is `VirTexModel.forward` + autograd
  * (virtex/models/captioning.py:71-143) executed by torch / torchvision library calls (SURVEY.md section 8b).
@@ -34,7 +34,7 @@ int vtx_version(void);
 int vtx_num_sms(void);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * tcgen05 GEMM:  D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )       bf16 x bf16 -> fp32 accumulate in TMEM
+ * wgmma GEMM:  D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )       bf16 x bf16 -> fp32 accumulate in registers
  * Replaces every cuBLASLt / cuDNN GEMM-shaped call on the path: nn.Linear fwd/dgrad/wgrad
  * (virtex/modules/textual_heads.py:168-170,199,245,277; torch/nn/modules/transformer.py:1158-1199) and the 1x1 /
  * im2col'd convolutions of torchvision Bottleneck (torchvision/models/resnet.py:146-158).
@@ -67,8 +67,8 @@ typedef struct VtxGemm {
   int32_t conv_n, conv_h, conv_w, conv_c;
   int32_t conv_mode; /* 0 = plain GEMM, 1 = implicit fprop/dgrad gather on A (64->64 channel problems run the halo-reuse
                         variant automatically), 2 = wgrad gather on B,
-                        4 = halo-reuse wgrad for C = Cout = 64: A = dy, B = x, D[9*C, Cout] fp32 += (atomic),
-                            i.e. the TRANSPOSE of mode 2's [Cout, 9*C] output,
+                        4 = wgrad for C = Cout = 64 in the transposed layout: A = dy, B = x, D[9*C, Cout] fp32 +=
+                            (atomic), i.e. the TRANSPOSE of mode 2's [Cout, 9*C] output,
                         5 = 7x7/2 stem fprop over the space-to-depth view S written by vtx_stem_s2d: A = S
                             [conv_n, conv_h + 3, conv_w + 3, 16] (conv_h x conv_w = OUTPUT size, conv_c = 64 = 4 pixels
                             x 16 channels), B = packed weights [64, 256] (vtx_stem_s2d_w_pack), D [n*h*w, 64] NHWC

@@ -1,4 +1,4 @@
-"""One-off cross-check (TEST INFRASTRUCTURE, needs /root/reference): checkpoints written by the UNMODIFIED reference
+"""One-off cross-check (TEST INFRASTRUCTURE, needs a reference checkout in $VIRTEX_REFERENCE_ROOT): checkpoints written by the UNMODIFIED reference
 (`virtex.utils.checkpointing.CheckpointManager` around its model + Lookahead(SGD) + LinearWarmupCosineAnnealingLR) load
 into virtex_b200's model and fused-optimiser state views, and checkpoints written by virtex_b200 load back into the
 reference objects (strict key match, momentum buffers bit-equal, schedule continues at the same learning rate).

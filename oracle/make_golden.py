@@ -1,4 +1,4 @@
-"""Generate tests/golden/*.pt by running the UNMODIFIED reference (imported from /root/reference) -- build container only.
+"""Generate tests/golden/*.pt by running the UNMODIFIED reference (a checkout named by $VIRTEX_REFERENCE_ROOT).
 
     python -m oracle.make_golden
 
@@ -180,7 +180,7 @@ def run_trainer_case():
 
 def main():
     if not ref_shim.available():
-        raise SystemExit("reference tree not found; goldens can only be regenerated in the build container")
+        raise SystemExit("reference tree not found: set VIRTEX_REFERENCE_ROOT to a checkout of the reference")
     warnings.filterwarnings("ignore")
     ref_shim.install()
     os.makedirs(GOLDEN_DIR, exist_ok=True)

@@ -1,16 +1,16 @@
-"""Import the UNMODIFIED reference (/root/reference) in this container -- TEST INFRASTRUCTURE ONLY.
+"""Import the UNMODIFIED reference (a checkout named by $VIRTEX_REFERENCE_ROOT) -- TEST INFRASTRUCTURE ONLY.
 
 The reference needs `albumentations` and `fvcore`, neither of which is installed here; both are irrelevant to the
 model math.  This shim injects inert stand-ins into `sys.modules` (SURVEY.md section 8c) so that
 `virtex.models.captioning`, `virtex.config.Config` and `virtex.factories` import and run unmodified.
-Used only by `oracle/make_golden.py`; /root/reference does not exist on the GPU box.
+Used only by `oracle/make_golden.py`; tests and the GPU path never need the reference.
 """
 import ast
 import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("VIRTEX_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("VIRTEX_REFERENCE_ROOT", "")
 
 
 class _CfgNode(dict):
@@ -92,6 +92,8 @@ class _CfgNode(dict):
 
 def install():
     """Make `import virtex` resolve to the reference tree with stubbed third-party deps."""
+    if not available():
+        raise RuntimeError("set VIRTEX_REFERENCE_ROOT to a checkout of the reference (kdexd/virtex)")
     if "albumentations" not in sys.modules:
         alb = types.ModuleType("albumentations")
 
@@ -119,4 +121,12 @@ def install():
 
 
 def available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "virtex"))
+    """True when $VIRTEX_REFERENCE_ROOT names a reference checkout OUTSIDE this repository (this repository's own
+    `virtex/` alias package must never stand in for the reference)."""
+    if not REFERENCE_ROOT:
+        return False
+    root = os.path.realpath(REFERENCE_ROOT)
+    here = os.path.realpath(os.path.join(os.path.dirname(os.path.abspath(__file__)), os.pardir))
+    if root == here or root.startswith(here + os.sep):
+        raise RuntimeError(f"VIRTEX_REFERENCE_ROOT={REFERENCE_ROOT} lies inside this repository, not in a reference checkout")
+    return os.path.isdir(os.path.join(root, "virtex"))

@@ -7,7 +7,7 @@ product (`virtex_b200/`) never does.
 
 Pinning: the reference ships no tests or golden vectors of its own (SURVEY.md section 8c) and its arithmetic lives
 in torch / torchvision.  This restatement is therefore pinned against the *live* reference modules imported from
-/root/reference in the build container (`oracle/make_golden.py`), and the resulting fixtures are committed under
+a reference checkout (`oracle/make_golden.py`), and the resulting fixtures are committed under
 `tests/golden/`; `tests/test_oracle_golden.py` re-checks the oracle against them everywhere.
 
 Reference call sites restated (file:line, relative to the reference root unless prefixed SP/ = site-packages):

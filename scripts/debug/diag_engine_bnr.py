@@ -53,9 +53,9 @@ def checked_gemm(A, Bm, D, M, N, K, **kw):
 
 E.gemm = checked_gemm
 eng.fuse_bn_reduce, eng.fuse_bn3_min_rows = True, 0
-for pair in ("0", "1"):
-    os.environ["VTX_GEMM_PAIR"] = pair
-    print(f"=== batch {B}, VTX_GEMM_PAIR={pair}")
+for dynamic in (False, True):
+    ops.set_dynamic_gemm_schedule(dynamic)
+    print(f"=== batch {B}, {'dynamic' if dynamic else 'static'} tile schedule")
     pending.clear()
     feat, h, w = eng.backbone_forward(batch["image"].cuda(), training=True)
     dfeat = (torch.randn(feat.shape, generator=torch.Generator().manual_seed(0)) * 0.01).bfloat16().cuda()

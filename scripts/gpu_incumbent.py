@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""The incumbent on the same B200: the reference's bicaptioning step as eager PyTorch (cuDNN convs, cuBLASLt linears,
+"""The incumbent on the same GPU: the reference's bicaptioning step as eager PyTorch (cuDNN convs, cuBLASLt linears,
 SDPA attention) under bf16 autocast.  Measurement infrastructure only -- nothing in `virtex_b200/` imports this.
 
-`/root/reference` does not exist on the GPU box, so the model is re-wired here from the library modules the reference
+The reference itself is not needed, so the model is re-wired here from the library modules the reference
 itself instantiates, exactly as it wires them:
   * torchvision `resnet50(zero_init_residual=True)` with `fc = Identity`, children run up to `layer4`
     (virtex/modules/visual_backbones.py:43-74);

@@ -151,7 +151,7 @@ def test_training_step_schedule(dry, spec_kw, batch_kw):
     assert names.count("vtx_cross_entropy") == 2 and names.count("vtx_embed_fwd") == 2
     assert names.count("vtx_attn_fwd") == 2 * 2 * spec.layers == names.count("vtx_attn_bwd")
     assert "vtx_stem_s2d" in names and "vtx_stem_im2col" not in names
-    # layer1's three 64 -> 64 3x3 convs use the halo-reuse wgrad
+    # layer1's three 64 -> 64 3x3 convs use the [(tap, cin), cout] wgrad (conv_mode 4)
     assert len([g for g in gemms if g[4] == 4]) == 3
     # BN-backward reductions: bn1 / bn2 of every block and bn3 of every block that is followed by an identity block and
     # has no downsample branch are accumulated by GEMM epilogues (a stride-2 conv2 dgrad is four GEMMs); stand-alone

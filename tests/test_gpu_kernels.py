@@ -5,7 +5,6 @@ through the C ABI (virtex_b200.ops.call).  Tolerances: bf16 outputs -> 1 bf16 ul
 tensor norm, and max-abs 2^-7 relative to the largest magnitude); fp32 reductions -> 1e-4 relative.
 """
 import math
-import os
 
 import pytest
 import torch
@@ -435,11 +434,11 @@ def test_gemm_masked_residual_epilogue():
 
 
 @pytest.mark.parametrize("M,N,K,tile_n", [
-    (60000, 64, 64, 0),      # 64-wide tiles: two independent 8-warp epilogue groups on alternate tiles, 3+ tiles per CTA
+    (60000, 64, 64, 0),      # 64-wide tiles, two staging buffers, 3+ tiles per CTA
     (19077, 64, 192, 0),     # same, ragged last M tile, odd tile count per CTA
-    (150, 64, 64, 0),        # two tiles in the whole launch: second group idle on most CTAs
-    (60000, 128, 64, 0),     # 128-wide: 16 epilogue warps, one chunk each
-    (40000, 256, 128, 0),    # 256-wide: 16 epilogue warps, two chunks each
+    (150, 64, 64, 0),        # two tiles in the whole launch: most CTAs idle
+    (60000, 128, 64, 0),     # 128-wide tiles
+    (40000, 256, 128, 0),    # 256-wide tiles
     (30011, 96, 64, 0),      # width that is not a multiple of 64
     (20000, 200, 64, 0),     # partial last column tile
     (30000, 256, 64, 128),   # forced 128-wide tiles over two column blocks (statistics flushed on block changes)
@@ -447,7 +446,7 @@ def test_gemm_masked_residual_epilogue():
     (9000, 2048, 64, 0),     # eight column blocks, 568 tiles: the tile counter hands most CTAs three or four tiles
 ])
 def test_gemm_epilogue_configurations_many_tiles(M, N, K, tile_n, schedule):
-    """Every epilogue configuration of gemm_tc_kernel (active warps / groups / staging buffers depend on the tile width)
+    """Every epilogue configuration of the GEMM kernel (wgmma width and staging buffers depend on the tile width)
     on launches with several tiles per CTA: output, BN statistics of the bf16-rounded output, and the packed residual path."""
     _need_cuda()
     ops = _ops()
@@ -529,8 +528,8 @@ def test_gemm_fused_bn_backward_reduce_plain(M, N, K, schedule):
 
 @pytest.mark.parametrize("NI,H,W,C", [(4, 14, 14, 128), (3, 56, 56, 64), (2, 30, 22, 64), (6, 7, 7, 256)])
 def test_gemm_fused_bn_backward_reduce_conv_dgrad(NI, H, W, C, schedule):
-    """The same through the implicit 3x3 dgrad (conv2 dgrad -> bn1), including the halo-reuse variant (C = 64) whose
-    partial spatial tiles have rows outside the image."""
+    """The same through the implicit 3x3 dgrad (conv2 dgrad -> bn1), including 64-channel layers whose partial
+    spatial tiles have rows outside the image."""
     _need_cuda()
     ops = _ops()
     g = torch.Generator().manual_seed(H * W + C)
@@ -612,16 +611,24 @@ def test_gemm_fused_bn_backward_reduce_over_residual_is_exact_for_every_tile_cou
                 _check_bnr(ops, D, y, bnp, sums, mask, bkeep if mask is not None else (y.float() * bnp[2] + bnp[3]) > 0)
 
 
-def _pair_env(on):
-    os.environ["VTX_GEMM_PAIR"] = "2" if on else "0"   # "2": pairs for every eligible shape, not only where they pay
+def _both_schedules(ops, run):
+    """run() under the static round-robin and the dynamic tile-counter schedule: {False: static, True: dynamic}."""
+    outs = {}
+    try:
+        for dynamic in (False, True):
+            ops.set_dynamic_gemm_schedule(dynamic)
+            outs[dynamic] = run()
+    finally:
+        ops.set_dynamic_gemm_schedule(False)
+    return outs
 
 
 @pytest.mark.parametrize("M,N,K", [(7680, 1024, 1024), (1000, 256, 512), (896, 10000, 256), (50176, 256, 1024), (641, 384, 320)])
 def test_gemm_cta_pairs_match_single_cta_and_torch(M, N, K):
-    """cta_group::2: a 2-CTA cluster runs one M = 256 MMA over two row tiles, each CTA staging half of the B tile.  Every
-    operand layout (K-major / MN-major A and B, split-K fp32 atomics), odd numbers of row tiles (the last pair's second CTA
-    is all padding), bias / activation / residual / statistics / fused BN-backward sums -- against the one-CTA-per-tile
-    path of the same library and torch."""
+    """Long-K and wide shapes that split into many tiles per CTA (the shapes the Blackwell build ran as 2-CTA pairs; every
+    tile is one CTA here): every operand layout (K-major / MN-major A and B, split-K fp32 atomics), a partial last row
+    tile, bias / activation / residual / statistics / fused BN-backward sums -- against torch, and the static tile
+    schedule against the dynamic tile counter, which hands the same tiles to CTAs in another order."""
     _need_cuda()
     ops = _ops()
     g = torch.Generator().manual_seed(M + N)
@@ -634,26 +641,24 @@ def test_gemm_cta_pairs_match_single_cta_and_torch(M, N, K):
     R = torch.randn(M, N, generator=g).bfloat16().cuda()
     y = (torch.randn(M, N, generator=g) * 1.5).bfloat16().cuda()
     bnp = _bnp(N, g)
-    outs = {}
-    try:
-        for pair in (False, True):
-            _pair_env(pair)
-            D1 = torch.empty(M, N, dtype=BF16, device="cuda")
-            st = torch.zeros(2, N, device="cuda")
-            ops.gemm(A, B, D1, M, N, K, stats=st)
-            D2 = torch.empty(M, N, dtype=BF16, device="cuda")
-            ops.gemm(A, Bt, D2, M, N, K, b_mn=1, bias=bias, act=1)
-            D3 = torch.zeros(M, N, dtype=BF16, device="cuda")
-            sums = torch.zeros(2, N, device="cuda")
-            if N % 32 == 0:
-                ops.gemm(A, Bt, D3, M, N, K, b_mn=1, residual=R, bnr=(y, bnp, sums, None))
-            D4 = torch.zeros(M, N, device="cuda")
-            if M % 8 == 0:
-                ops.gemm(At, Bt, D4, M, N, K, a_mn=1, b_mn=1, atomic=True, split_k=2, out_f32=True)
-            outs[pair] = (D1, st, D2, D3, sums, D4)
-    finally:
-        os.environ.pop("VTX_GEMM_PAIR", None)
-    D1, st, D2, D3, sums, D4 = outs[True]
+
+    def run():
+        D1 = torch.empty(M, N, dtype=BF16, device="cuda")
+        st = torch.zeros(2, N, device="cuda")
+        ops.gemm(A, B, D1, M, N, K, stats=st)
+        D2 = torch.empty(M, N, dtype=BF16, device="cuda")
+        ops.gemm(A, Bt, D2, M, N, K, b_mn=1, bias=bias, act=1)
+        D3 = torch.zeros(M, N, dtype=BF16, device="cuda")
+        sums = torch.zeros(2, N, device="cuda")
+        if N % 32 == 0:
+            ops.gemm(A, Bt, D3, M, N, K, b_mn=1, residual=R, bnr=(y, bnp, sums, None))
+        D4 = torch.zeros(M, N, device="cuda")
+        if M % 8 == 0:
+            ops.gemm(At, Bt, D4, M, N, K, a_mn=1, b_mn=1, atomic=True, split_k=2, out_f32=True)
+        return D1, st, D2, D3, sums, D4
+
+    outs = _both_schedules(ops, run)
+    D1, st, D2, D3, sums, D4 = outs[False]
     assert rel(D1, ref) < 4e-3 and rel(D2, torch.relu(ref + bias)) < 4e-3
     assert rel(st[0], D1.double().sum(0)) < 1e-4 and rel(st[1], (D1.double() ** 2).sum(0)) < 1e-4
     if N % 32 == 0:
@@ -661,14 +666,15 @@ def test_gemm_cta_pairs_match_single_cta_and_torch(M, N, K):
         _check_bnr(ops, D3, y, bnp, sums, None, (y.float() * bnp[2] + bnp[3]) > 0)
     if M % 8 == 0:
         assert rel(D4, ref) < 1e-4
-    for a, b in zip(outs[True], outs[False]):
+    for a, b in zip(outs[False], outs[True]):
         assert rel(a, b) < (2e-3 if a.dtype == BF16 else 1e-4)   # (bf16: at most a few last-bit flips)
 
 
 @pytest.mark.parametrize("NI,H,W,C,Cout", [(16, 14, 14, 256, 256), (9, 7, 7, 512, 512), (5, 28, 28, 128, 128)])
 def test_gemm_cta_pairs_implicit_conv(NI, H, W, C, Cout):
-    """CTA pairs through the implicit 3x3 convolution modes: fprop (4-D activation boxes per CTA, half of the K-major
-    weight tile each) and wgrad (each CTA gathers the taps of its half of the (tap, cin) columns)."""
+    """The implicit 3x3 convolution modes on 128- to 512-channel layers (the shapes the Blackwell build ran as 2-CTA
+    pairs): fprop (4-D activation boxes, K-major weight tiles, BN statistics) and split-K wgrad (every 64-column atom of
+    the (tap, cin) columns gathered by its own box) -- against torch, under both tile schedules."""
     _need_cuda()
     ops = _ops()
     g = torch.Generator().manual_seed(H + C)
@@ -676,20 +682,18 @@ def test_gemm_cta_pairs_implicit_conv(NI, H, W, C, Cout):
     x = (torch.randn(NI, H, W, C, generator=g) * 0.5).bfloat16().cuda()
     w = (torch.randn(Cout, 3, 3, C, generator=g) * 0.03).bfloat16().cuda()
     dy = (torch.randn(NI, H, W, Cout, generator=g) * 0.5).bfloat16().cuda()
-    outs = {}
-    try:
-        for pair in (False, True):
-            _pair_env(pair)
-            yo = torch.empty(M, Cout, dtype=BF16, device="cuda")
-            st = torch.zeros(2, Cout, device="cuda")
-            ops.gemm(x, w.view(Cout, 9 * C), yo, M, Cout, 9 * C, lda=C, stats=st, conv=(NI, H, W, C), conv_mode=1)
-            dw = torch.zeros(Cout, 9 * C, device="cuda")
-            ops.gemm(dy, x, dw, Cout, 9 * C, M, atomic=True, split_k=2, lda=Cout, ldb=C, conv=(NI, H, W, C), conv_mode=2,
-                     out_f32=True)
-            outs[pair] = (yo, st, dw)
-    finally:
-        os.environ.pop("VTX_GEMM_PAIR", None)
-    yo, st, dw = outs[True]
+
+    def run():
+        yo = torch.empty(M, Cout, dtype=BF16, device="cuda")
+        st = torch.zeros(2, Cout, device="cuda")
+        ops.gemm(x, w.view(Cout, 9 * C), yo, M, Cout, 9 * C, lda=C, stats=st, conv=(NI, H, W, C), conv_mode=1)
+        dw = torch.zeros(Cout, 9 * C, device="cuda")
+        ops.gemm(dy, x, dw, Cout, 9 * C, M, atomic=True, split_k=2, lda=Cout, ldb=C, conv=(NI, H, W, C), conv_mode=2,
+                 out_f32=True)
+        return yo, st, dw
+
+    outs = _both_schedules(ops, run)
+    yo, st, dw = outs[False]
     ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float().permute(0, 3, 1, 2), padding=1).permute(0, 2, 3, 1).reshape(M, Cout)
     assert rel(yo, ref) < 4e-3
     assert rel(st[0], yo.double().sum(0)) < 1e-4

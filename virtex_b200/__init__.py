@@ -1,2 +1,2 @@
-"""virtex_b200 -- B200-native (sm_100a) implementation of the VirTex bicaptioning pretraining step."""
+"""virtex_b200 -- H100-native (sm_90a) implementation of the VirTex bicaptioning pretraining step."""
 __version__ = "0.1.0"

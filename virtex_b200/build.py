@@ -1,4 +1,4 @@
-"""In-tree build of libvirtex_b200.so (sm_100a only).
+"""In-tree build of libvirtex_b200.so (sm_90a only).
 
 `python -m virtex_b200.build` compiles every `csrc/*.cu` with nvcc (cross-compiles without a GPU) and links
 them into `virtex_b200/libvirtex_b200.so`, next to this file, so that the built library travels with the
@@ -17,7 +17,7 @@ OBJ_DIR = os.path.join(ROOT, "build", "obj")
 LIB_PATH = os.path.join(HERE, "libvirtex_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-DVTX_NO_FAST_MATH",  # no --use_fast_math: erff / division accuracy matters for parity
     "-I", os.path.join(ROOT, "include"),
 ]

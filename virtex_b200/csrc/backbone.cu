@@ -1,5 +1,5 @@
 // Memory-bound kernels of the ResNet backbone (NHWC bf16 activations, fp32 statistics).
-// They surround the tcgen05 GEMM (gemm_tc.cu): train-mode BatchNorm finalize/apply/backward, ReLU, residual add,
+// They surround the wgmma GEMM (gemm_tc.cu): train-mode BatchNorm finalize/apply/backward, ReLU, residual add,
 // stem im2col + fused BN/ReLU/max-pool, strided-conv gathers, and conv-weight layout transforms.
 // Reference semantics: torchvision/models/resnet.py:143-163 (Bottleneck), :268-276 (stem), nn.BatchNorm2d train mode
 // (SURVEY.md Appendix C.2): biased variance for normalisation, unbiased for running_var, momentum 0.1, eps 1e-5.
@@ -330,9 +330,8 @@ struct BnFwdFold {
   int training;
 };
 
-// kUa = independent 16-byte loads per tensor in flight per thread.  Measured on B200 (r02_bn_attn.ncu-rep): ~32 KB in
-// flight per SM (one input tensor at kUa = 4) caps the kernel at ~3.9 TB/s, ~64 KB reaches ~5.9 TB/s -- so the
-// single-input variants (no residual operand) run 8 loads deep.
+// kUa = independent 16-byte loads per tensor in flight per thread: HBM bandwidth needs many bytes in flight per SM, so
+// the single-input variants (no residual operand) run 8 loads deep.
 template <bool kFold, int kUa>
 __global__ void __launch_bounds__(256, 2) bn_act_kernel(const __nv_bfloat16* __restrict__ y, float* __restrict__ bnp,
                               const __nv_bfloat16* __restrict__ res, const float* __restrict__ bnp_res,
@@ -423,8 +422,7 @@ __global__ void __launch_bounds__(256, 2) bn_act_kernel(const __nv_bfloat16* __r
 // stem: pooled[n,ph,pw,:] = max over the 3x3/stride 2/pad 1 window of relu(y*scale+shift); idx = window slot of the max
 // Row-per-block form of the kernel below for C/8 dividing 256 (every ResNet stem): one CTA walks pooled rows (n, ph);
 // a thread keeps its channel group and BN coefficients for the whole launch and steps pw by blockDim / (C/8), so the loop has
-// no division at all (the flat-index form spent ~400 of its ~900 instructions per item on five 64-bit div / mod:
-// 0.284 ms for 0.54 GB, profiles/r02f_launches_step.csv).
+// no division at all (the flat-index form spent ~400 of its ~900 instructions per item on five 64-bit div / mod).
 __global__ void __launch_bounds__(256) bn_relu_maxpool_rows_kernel(const __nv_bfloat16* __restrict__ y,
                                                                    const float* __restrict__ bnp,
                                                                    __nv_bfloat16* __restrict__ out,
@@ -569,8 +567,8 @@ __global__ void maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dpool, cons
   }
 }
 
-// (A shared-memory tiled variant of the FORWARD pool was measured in round 2 and deleted: 0.42 ms against 0.28 ms for
-// the direct kernel above -- the ~2.25x re-normalisation it saved is cheaper than its staging pass.)
+// (A shared-memory tiled variant of the FORWARD pool was slower than the direct kernel above and deleted: the ~2.25x
+// re-normalisation it saved is cheaper than its staging pass.)
 // same arithmetic as maxpool_bwd_kernel, but a CTA first stages the kTP + 1 pooled rows
 // (gradients + argmax slots) it needs in shared memory with linear coalesced copies and then produces 2 * kTP input
 // rows from them.  The validated kernel gathers every pooled element from L2 up to nine times (1.4 GB of L2 -> SM

@@ -28,10 +28,10 @@ extern "C" int vtx_sizeof_gemm(void) { return (int)sizeof(VtxGemm); }
 extern "C" int vtx_num_sms(void) {
   static int sms[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (sms[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
     sms[dev] = v;
   }
   return sms[dev];

@@ -1,37 +1,27 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a -- the one tensor-core kernel behind every GEMM-shaped op of the
-// VirTex bicaptioning step (1x1 convs, implicit 3x3 convs, im2col'd strided convs, all nn.Linear fwd/dgrad/wgrad,
-// vocabulary projection).  See include/virtex_b200.h (VtxGemm) for the contract.
+// wgmma / TMA GEMM for sm_90a -- the one tensor-core kernel behind every GEMM-shaped op of the VirTex bicaptioning
+// step (1x1 convs, implicit 3x3 convs, im2col'd strided convs, all nn.Linear fwd/dgrad/wgrad, vocabulary projection).
+// See include/virtex_b200.h (VtxGemm) for the contract.
 //
-// Structure (persistent, warp specialised, one CTA per SM, 640 threads):
-//   warp 0 : TMA producer   (one elected lane)  global -> 128B-swizzled smem ring of (A 16 KB, B = tile_n*128 B) stages;
-//                           the ring depth is whatever fits next to the output staging tile (2..8 stages); it also owns
-//                           the tile schedule: every tile index (static round robin, or fetched from a per-launch atomic
-//                           counter) is published to the other roles through a small index ring in shared memory
-//   warp 1 : MMA issuer     tcgen05.mma.kind::f16, M=128, N=tile_n, K=16 per issue; the whole warp walks the schedule
-//                           (uniform-datapath descriptors), one elect.sync lane issues
-//   warp 2 : TMEM allocator (512 columns = 2 accumulator stages of up to 256 fp32 columns)
-//   warps 4-19 : epilogue   tcgen05.ld -> bias / residual / activation -> bf16 tile in 128B-swizzled smem (TMEM is
-//                           released to the MMA warp here) -> one elected thread issues TMA stores (cp.async.bulk.tensor,
-//                           out-of-bounds rows/columns clipped by the hardware); a statistics pass over the staged tile
-//                           accumulates, in registers across the CTA's tiles, either the BN batch statistics of a conv
-//                           output or (kBnr) the BN-BACKWARD sums of a gradient.  With two staging buffers (short K
-//                           loops) the warps form two independent groups working on alternate tiles.  (fp32 / split-K
-//                           outputs skip staging: red.global.add.v4.f32 straight from registers.)
-// CTA pairs (kPair, cta_group::2): for long K loops the kernel is launched in 2-CTA clusters; one M = 256 MMA per K step
-// is issued by the leader CTA over the two CTAs' shared memories (own 128 rows of A and HALF of the B tile each, loaded
-// with the .cta_group::2 TMA form that signals the leader's barrier), commits are multicast to both CTAs' barriers, each
-// CTA's epilogue drains its own 128 accumulator lanes and releases them on the leader's barrier (remote mbarrier arrive).
-// Four mbarrier pipelines: smem full/empty (TMA <-> MMA), tmem full/empty (MMA <-> epilogue), residual landed, and the
-// tile-index ring (producer <-> MMA warp and epilogue groups).
+// Structure (persistent, warp specialised, one CTA per SM, 384 threads = three warpgroups):
+//   warpgroup 0 : TMA producer (one thread)  global -> 128B-swizzled smem ring of (A 16 KB, B = tile_n*128 B) stages;
+//                 the ring depth is whatever fits next to the output staging tile (2..8 stages); it also owns the tile
+//                 schedule: every tile index (static round robin, or fetched from a per-launch atomic counter) is
+//                 published to the consumers through a small index ring in shared memory.  It hands most of its
+//                 registers to the consumers (setmaxnreg).
+//   warpgroups 1, 2 : MMA + epilogue, rows [0, 64) and [64, 128) of the 128-row tile: wgmma.mma_async m64nNk16
+//                 (N = tile_n in {64, 128, 192, 256}) with fp32 accumulators in registers, then bias / residual /
+//                 activation -> bf16 tile in 128B-swizzled smem -> one thread issues TMA stores (cp.async.bulk.tensor,
+//                 out-of-bounds rows/columns clipped by the hardware); a statistics pass over the staged tile
+//                 accumulates, in registers across the CTA's tiles, either the BN batch statistics of a conv output or
+//                 (p.bnr) the BN-BACKWARD sums of a gradient.  (fp32 / split-K outputs skip staging: stores or fp32
+//                 atomics straight from registers.)
+// Three mbarrier pipelines: smem full/empty (TMA <-> MMA), residual landed, and the tile-index ring.
 //
-// Operand "major-ness" is a runtime property (instruction-descriptor bits + smem descriptor strides), so the same
-// kernel serves fprop (A,B K-major), dgrad (B MN-major) and wgrad (A,B MN-major) without transposing activations.
-// conv_mode 1/2 replace the 2D TMA loads by 4D NHWC box loads whose out-of-bounds elements are zero-filled by the
-// TMA unit: that *is* the im2col of a 3x3/stride-1/pad-1 convolution, with no extra HBM traffic.
-// 64 -> 64 channel 3x3 convs (ResNet layer1) additionally have halo-reuse variants that fetch the input ONCE per
-// 8 x 16 spatial tile and address the nine taps as row-shifted descriptor views of that tile: mode 3 (fprop / dgrad,
-// selected automatically from mode 1; weights stationary in shared memory) and mode 4 (wgrad; accumulators stay in
-// TMEM across all spatial tiles of the CTA).
+// Operand "major-ness" is a runtime property (wgmma transpose bits + smem descriptor strides), so the same kernel serves
+// fprop (A,B K-major), dgrad (B MN-major) and wgrad (A,B MN-major) without transposing activations.
+// conv_mode 1/2 replace the 2D TMA loads by 4D NHWC box loads whose out-of-bounds elements are zero-filled by the TMA
+// unit: that *is* the im2col of a 3x3/stride-1/pad-1 convolution, with no extra HBM traffic.  conv_mode 4 (the
+// [(tap, cin), cout] weight gradient of a 64 -> 64 3x3 conv) runs as conv_mode 2 with a transposed fp32 store.
 #include <stdlib.h>
 #include "ptx.cuh"
 #include "vtx_common.cuh"
@@ -50,16 +40,10 @@ constexpr int kBM = 128;
 constexpr int kBK = 64;
 constexpr int kMaxStages = 8;
 constexpr int kABytes = kBM * kBK * 2;        // 16384
-constexpr int kSmemTotal = 232448;            // 227 KB: the per-CTA maximum on sm_100
-constexpr int kCtrlBytes = 1024;              // barriers + TMEM slot, placed right after the 1024-aligned base
-// Up to 16 epilogue warps (4 TMEM lane quadrants x up to 4 column-chunk groups) at 96 registers each.  The round-2
-// profile showed the 8-warp / 168-register epilogue LATENCY bound on the short-K convs (issue slots 40 % busy, DRAM
-// 40 %, two warps per scheduler): with four warps per scheduler the 256- and 128-wide tiles run 8-12 % faster.  Tiles
-// narrower than 128 columns have only two chunks, so those launches keep 8 active warps (p.epi_warps; the idle ones
-// only cost barrier width: 64-wide tiles measured 10 % SLOWER with all 16 in the barriers).
-constexpr int kEpiWarps = 16;
-constexpr int kThreads = 128 + 32 * kEpiWarps;
-constexpr int kHaloH = 18, kHaloW = 10;  // modes 3/4: halo of an 8 (w) x 16 (h) tile = 18 lines x 10 pixels x 64 ch (bf16)
+constexpr int kSmemTotal = 232448;            // 227 KB: the per-block maximum on sm_90
+constexpr int kCtrlBytes = 1024;              // barriers + tile-index ring, placed right after the 1024-aligned base
+constexpr int kThreads = 384;                 // producer warpgroup + two MMA / epilogue warpgroups
+constexpr int kEpiThreads = 256;
 
 // x / d for 0 <= x < 2^31 and the launch-invariant divisor d: (umulhi(x, mul) >> shr), d == 1 handled apart
 struct FastDiv {
@@ -96,11 +80,7 @@ struct GemmKParams {
   int out_f32, atomic, act;
   int stages, stage_bytes;   // smem ring depth / bytes per stage
   int cbytes, nbuf;          // bytes of one bf16 staging buffer (0: no staging) / number of staging buffers
-  int epi_warps, epi_groups; // active epilogue warps (8 or 16) / independent groups they form (2 for staged 64-wide tiles)
   int res_tma;               // residual tile is TMA-loaded into the staging buffer and added there
-  int bstat_bytes;           // mode 3: bytes of the stationary weight region (0 otherwise)
-  int halo_w;                // modes 3/4: pixels per halo line in shared memory
-  int dy_off;                // mode 4: byte offset of the dy tile inside a stage (1024-aligned)
   float alpha;
   void* D;
   long long ldd;
@@ -120,47 +100,40 @@ struct GemmKParams {
   // atomic on its way out.  With a static round-robin schedule an SM that is held by somebody else's CTA (NCCL's
   // all-reduce kernels during the overlapped gradient exchange) delays ITS fixed share of tiles to the end of every GEMM
   // issued meanwhile; here the CTAs that do run drain the counter and a late CTA finds nothing left.
-  // nullptr: static schedule (mode 4, single-GPU default -- see vtx_gemm_set_dynamic_schedule).
+  // nullptr: static schedule (single-GPU default -- see vtx_gemm_set_dynamic_schedule).
   unsigned int* sched;
   unsigned int sched_base;
   int sched_chunk;
   int nt_major;
-  // BN-backward reduction fused into the epilogue (kBnr kernel; `stats` then holds the [2, N] sums of dz and dz * xhat):
+  // BN-backward reduction fused into the epilogue (bnr != 0; `stats` then holds the [2, N] sums of dz and dz * xhat):
   // y has the geometry of D -- row stride bnr_ldy for plain GEMMs, (w, h, n) strides for implicit-conv outputs and views
   const __nv_bfloat16* bnr_y;
   const float* bnr_bnp;      // [4, N]: mean, invstd, scale, shift of the BN whose output gradient D is
   const uint8_t* bnr_mask;   // optional ReLU bit mask [M, N/8] (plain GEMMs); nullptr: mask recomputed from y
   long long bnr_ldy, bnr_sw, bnr_sh, bnr_sn;
   int vW, vH;                // extent of the output (view) grid of the implicit-conv modes
-  int bnr_prefetch;          // pull the y tile into L2 with a TMA prefetch when the tile's epilogue starts
-  // CTA pair (kPair kernel, cta_group::2): a 2-CTA cluster works on two vertically adjacent 128-row tiles with ONE
-  // M = 256 MMA per K step; each CTA stages its own A tile and half of the B tile, so every SM pulls 1.5x fewer operand
-  // bytes through L2 and shared memory per flop.  The schedule then runs over m_sched = ceil(m_tiles / 2) row-tile pairs.
-  int pair, m_sched;              // tile index runs over row tiles first (BN statistics: a CTA's column block changes rarely)
+  int bnr_prefetch;          // pull the y tile into L2 with a TMA prefetch when the tile starts
+  int bnr;                   // 0: plain statistics (or none), 1: BN-backward sums, ReLU mask from y, 2: from a bit mask
+  int trans_d;               // fp32 output stored transposed: D[col * ldd + row] (conv_mode 4)
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 __device__ __forceinline__ void epi_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // schedule index -> (split, row tile, column tile)
-// (`rank`: this CTA's rank in its pair -- the pair shares the schedule index, rank r owns row tile 2 * index + r)
-__device__ __forceinline__ void decode_tile(const GemmKParams& p, int t, int& ks, int& mt, int& nt, int rank = 0) {
+__device__ __forceinline__ void decode_tile(const GemmKParams& p, int t, int& ks, int& mt, int& nt) {
   ks = fdiv(t, p.d_mn);
-  const int rem = t - ks * (p.m_sched * p.n_tiles);
+  const int rem = t - ks * (p.m_tiles * p.n_tiles);
   if (p.nt_major) {
     nt = fdiv(rem, p.d_mt);
-    mt = rem - nt * p.m_sched;
+    mt = rem - nt * p.m_tiles;
   } else {
     mt = fdiv(rem, p.d_nt);
     nt = rem - mt * p.n_tiles;
   }
-  if (p.pair) mt = 2 * mt + rank;
 }
 __device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
@@ -190,274 +163,152 @@ __device__ __forceinline__ uint32_t add_res_bf16x2(float lo, float hi, uint32_t 
   const __nv_bfloat162 o = __hadd2(a, r);
   return *reinterpret_cast<const uint32_t*>(&o);
 }
-__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
-  uint32_t d;
-  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
-  return d;
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
-// One 32-column chunk of one row: staged residual (4 x 16 B, swizzled) + accumulators -> staged output, in place.
-// The ReLU bit mask (bit c of `mb` <-> column c) becomes a per-pair AND mask with ONE byte-permute per pair: prmt's
-// sign-replicate mode turns the top bit of a byte into 0x00 / 0xff, and the 8 shifted copies mb << s put every mask
-// bit at the top of some byte.  ~2 instructions per element where unpack + select + fp32 add + repack took ~4.5.
-template <bool kMask>
-__device__ __forceinline__ void residual_chunk_packed(const float* v, uint32_t sp, int cb, int sw, uint32_t mb, bool dead) {
-  uint32_t xs[8];
-  if (kMask) {
-#pragma unroll
-    for (int s_ = 0; s_ < 8; ++s_) xs[s_] = mb << s_;
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint32_t addr = sp + (((cb + i) ^ sw) << 4);
-    const uint4 raw = lds128(addr);
-    const uint32_t rw[4] = {raw.x, raw.y, raw.z, raw.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      uint32_t r = rw[k];
-      if (kMask) {
-        // columns 8i + 2k (bit 2k of byte i) and 8i + 2k + 1
-        const uint32_t sel = ((0xCu + i) << 12) | ((0xCu + i) << 8) | ((0x8u + i) << 4) | (0x8u + i);
-        r &= prmt(xs[7 - 2 * k], xs[6 - 2 * k], sel);
-      }
-      o[k] = dead ? 0u : add_res_bf16x2(v[8 * i + 2 * k], v[8 * i + 2 * k + 1], r);
-    }
-    sts128(addr, o[0], o[1], o[2], o[3]);
-  }
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// fp32 epilogue math on one 32-column chunk of one accumulator row
-__device__ __forceinline__ void epi_math(float* v, const GemmKParams& p, long long grow, int col0, bool full) {
-  if (p.alpha != 1.0f) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] *= p.alpha;
-  }
-  if (p.bias != nullptr) {
-    if (full) {
-#pragma unroll
-      for (int i = 0; i < 32; i += 4) {
-        const float4 b = *reinterpret_cast<const float4*>(p.bias + col0 + i);
-        v[i] += b.x; v[i + 1] += b.y; v[i + 2] += b.z; v[i + 3] += b.w;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (col0 + i < p.N) v[i] += p.bias[col0 + i];
-    }
-  }
-  if (p.residual != nullptr && !p.res_tma && grow >= 0) {
-    const __nv_bfloat16* rp = p.residual + grow * p.ldr + col0;
-    // res_mask requires N % 32 == 0 (checked on the host), so a masked chunk is always full
-    const uint32_t mb = p.res_mask ? *reinterpret_cast<const uint32_t*>(p.res_mask + (grow * p.N + col0) / 8) : 0xffffffffu;
-    if (full) {
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        const uint4 u = *reinterpret_cast<const uint4*>(rp + i);
-        const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = __bfloat1622float2(h2[j]);
-          v[i + 2 * j] += ((mb >> (i + 2 * j)) & 1u) ? f.x : 0.f;
-          v[i + 2 * j + 1] += ((mb >> (i + 2 * j + 1)) & 1u) ? f.y : 0.f;
-        }
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (col0 + i < p.N) v[i] += __bfloat162float(rp[i]);
-    }
-  }
-  if (p.act == 1) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-  } else if (p.act == 2) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
-  }
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_bn(float* d, uint64_t ad, uint64_t bd, uint32_t accumulate) {
+  if constexpr (BN == 64) wgmma_n64<TA, TB>(d, ad, bd, accumulate);
+  else if constexpr (BN == 128) wgmma_n128<TA, TB>(d, ad, bd, accumulate);
+  else if constexpr (BN == 192) wgmma_n192<TA, TB>(d, ad, bd, accumulate);
+  else wgmma_n256<TA, TB>(d, ad, bd, accumulate);
 }
 
-// registers -> global for fp32 outputs (plain or atomic accumulate)
-__device__ __forceinline__ void epi_store_f32(const float* v, const GemmKParams& p, long long grow, int col0, bool full) {
-  float* op = reinterpret_cast<float*>(p.D) + grow * p.ldd + col0;
-  if (p.atomic) {
-    if (full) {
+// K loop of one tile for one consumer warpgroup (rows [64 wg, 64 wg + 64) of the tile): one wgmma m64nBNk16 per 16-deep
+// K step, one commit group per stage.  A stage is handed back to the producer (one arrive per warpgroup) as soon as the
+// MMAs of the NEXT stage are issued and the ones reading it have completed, so one stage's MMAs are always in flight
+// while the warpgroup waits for the following stage.
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void mma_tile(float* acc, uint8_t* smem, const GemmKParams& p, int kb0, int kb1, int wg,
+                                         uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                         bool signal) {
+  constexpr uint32_t a_step = TA ? 2048u : 32u;  // 16 k: two 8-row groups (MN-major) / 32 bytes along a row (K-major)
+  constexpr uint32_t b_step = TB ? 2048u : 32u;
+  constexpr uint32_t a_lbo = TA ? 8192u : 16u;
+  constexpr uint32_t b_lbo = TB ? 8192u : 16u;
+  int prev = -1;
 #pragma unroll
-      for (int i = 0; i < 32; i += 4) red_add_v4(op + i, v[i], v[i + 1], v[i + 2], v[i + 3]);
-    } else {
+  for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t s0 = smem_u32(smem + stage * p.stage_bytes);
+    const uint32_t sA = s0 + (uint32_t)wg * 8192u;  // 64 rows (K-major) or the wg-th 64-row atom (MN-major)
+    const uint32_t sB = s0 + (uint32_t)kABytes;
+    wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (col0 + i < p.N) atomicAdd(op + i, v[i]);
-    }
-  } else if (full) {
-#pragma unroll
-    for (int i = 0; i < 32; i += 4) *reinterpret_cast<float4*>(op + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 32; ++i)
-      if (col0 + i < p.N) op[i] = v[i];
+    for (int k = 0; k < kBK / 16; ++k)
+      wgmma_bn<BN, TA, TB>(acc, make_wgmma_desc(sA + k * a_step, a_lbo, 1024),
+                           make_wgmma_desc(sB + k * b_step, b_lbo, 1024), (kb > kb0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && signal) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == p.stages) { stage = 0; phase ^= 1; }
   }
+  wgmma_wait<0>();
+  if (prev >= 0 && signal) mbar_arrive(&empty_bar[prev]);
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
 }
 
-#define LOAD2D(...) (kPair ? tma_load_2d_pair(__VA_ARGS__) : tma_load_2d(__VA_ARGS__))
-#define LOAD4D(...) (kPair ? tma_load_4d_pair(__VA_ARGS__) : tma_load_4d(__VA_ARGS__))
-// kBnr (1: ReLU mask recomputed from y, 2: ReLU bit mask): the statistics pass over the staged output tile computes the BATCH-NORM BACKWARD sums instead of sum / sum of
-// squares: this GEMM's output is the gradient dA w.r.t. a BN(+ReLU) output, and  sum_m dz,  sum_m dz * xhat  with
-// dz = dA * [ReLU mask], xhat = (y - mean) * invstd  used to be a separate pass over dA and y (vtx_bn_bwd_reduce).  The
-// y tile is pulled into L2 by a TMA prefetch when the tile's epilogue starts and read with 16-byte loads in the pass.
-template <int kBnr, int kPair>
+// p.bnr (1: ReLU mask recomputed from y, 2: ReLU bit mask): the statistics pass over the staged output tile computes the
+// BATCH-NORM BACKWARD sums instead of sum / sum of squares: this GEMM's output is the gradient dA w.r.t. a BN(+ReLU)
+// output, and  sum_m dz,  sum_m dz * xhat  with dz = dA * [ReLU mask], xhat = (y - mean) * invstd  used to be a separate
+// pass over dA and y (vtx_bn_bwd_reduce).  The y tile is pulled into L2 by a TMA prefetch when the tile starts and read
+// with 16-byte loads in the pass.
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
-               const __grid_constant__ CUtensorMap tmY, const GemmKParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
+                  const __grid_constant__ CUtensorMap tmY, const GemmKParams p) {
   VTX_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(base);
   uint64_t* full_bar = bars;                     // [kMaxStages]
   uint64_t* empty_bar = bars + kMaxStages;       // [kMaxStages]
-  uint64_t* tfull_bar = bars + 2 * kMaxStages;   // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;          // [2]
-  uint64_t* res_bar = tempty_bar + 2;            // [2] residual tile landed in staging buffer b
-  uint64_t* bst_bar = res_bar + 2;               // [1] stationary weights landed (mode 3)
-  uint64_t* sch_full = bst_bar + 1;              // [kSched] tile index published
-  uint64_t* sch_empty = sch_full + kSched;       // [kSched] tile index read by the MMA warp and the epilogue group that owns the slot
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sch_empty + kSched);
-  volatile int* sch_tile = reinterpret_cast<volatile int*>(tmem_slot + 2);  // [kSched]
+  uint64_t* res_bar = bars + 2 * kMaxStages;     // [2] residual tile landed in staging buffer b
+  uint64_t* sch_full = res_bar + 2;              // [kSched] tile index published
+  uint64_t* sch_empty = sch_full + kSched;       // [kSched] tile index read by every consumer thread
+  volatile int* sch_tile = reinterpret_cast<volatile int*>(sch_empty + kSched);  // [kSched]
   uint8_t* smem = base + kCtrlBytes;                       // stage ring (1024-aligned)
-  uint8_t* bstat = smem + p.stages * p.stage_bytes;        // mode 3: stationary weights [9 taps][bn rows][128 B]
-  uint8_t* cstage0 = bstat + p.bstat_bytes;                // bf16 staging: nbuf x [bn/64 slabs][128 rows][128 B], SW128
+  uint8_t* cstage0 = smem + p.stages * p.stage_bytes;      // bf16 staging: nbuf x [bn/64 slabs][128 rows][128 B], SW128
 
   // broadcast from lane 0 so that the compiler sees the warp index (and every role branch on it) as warp-uniform
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int total_tiles = p.m_sched * p.n_tiles * p.k_splits;
-  // schedule identity: a CTA, or a CTA pair (the two CTAs of a pair walk the same static schedule)
-  const int rank = kPair ? (int)cluster_ctarank() : 0;
-  const int sched_id = kPair ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int sched_n = kPair ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int total_tiles = p.m_tiles * p.n_tiles * p.k_splits;
   const int nstages = p.stages;
 
   // the producer thread's first tile: requested before anything else (the counter belongs to this launch alone, so it
   // need not wait for the previous kernel) and consumed after the prologue
-  int t_first = sched_id;
+  int t_first = blockIdx.x;
   if (warp == 0 && lane == 0) {
     if (p.sched != nullptr) t_first = (int)(atomicAdd(p.sched, 1u) - p.sched_base) * p.sched_chunk;
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (p.cbytes) tma_prefetch_desc(&tmD);
     if (p.res_tma) tma_prefetch_desc(&tmR);
-    if (kBnr) tma_prefetch_desc(&tmY);
+    if (p.bnr) tma_prefetch_desc(&tmY);
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < nstages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], (kPair ? 2 : 1) * (p.epi_warps * 32 / p.epi_groups));  // pair: both CTAs' epilogues
-      mbar_init(&res_bar[i], 1);
-    }
-    mbar_init(bst_bar, 1);
+    for (int i = 0; i < 2; ++i) mbar_init(&res_bar[i], 1);
     for (int i = 0; i < kSched; ++i) {
       mbar_init(&sch_full[i], 1);
-      mbar_init(&sch_empty[i], 1 + p.epi_warps * 32 / p.epi_groups);
+      mbar_init(&sch_empty[i], kEpiThreads);
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (kPair) {
-      tmem_alloc_pair(tmem_slot, 512);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_slot, 512);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  // pair: the peer's barriers must exist before the leader's MMA commits / this CTA's TMA loads signal across the pair
-  if (kPair) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   VTX_PDL_WAIT();  // everything above overlapped the previous kernel's tail; its results are visible from here
 
-  const int bn_cta = kPair ? (p.bn >> 1) : p.bn;  // B rows staged by this CTA
-  const uint32_t b_bytes = (uint32_t)bn_cta * kBK * 2;
-
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================================================== TMA producer (warpgroup 0, one thread)
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      const uint32_t b_bytes = (uint32_t)p.bn * kBK * 2;
       int stage = 0;
       uint32_t phase = 0;
-      // modes 0-3: every tile index goes through the ring, whether it came from the counter or from the static schedule;
-      // two end markers (>= total_tiles) close it, one per epilogue group
-      int t = t_first, sit = 0, ends = 0;
+      // every tile index goes through the ring, whether it came from the counter or from the static schedule; one end
+      // marker (>= total_tiles) closes it
+      int t = t_first, sit = 0;
       // tile after `t_`: the next one of the current chunk, else the first one of a freshly fetched chunk (dynamic), or
       // the CTA's next round-robin tile (static)
       auto next_after = [&](int t_) -> int {
-        if (p.sched == nullptr) return t_ + sched_n;
+        if (p.sched == nullptr) return t_ + (int)gridDim.x;
         if ((t_ + 1) % p.sched_chunk != 0 && t_ + 1 < total_tiles) return t_ + 1;
         return (int)(atomicAdd(p.sched, 1u) - p.sched_base) * p.sched_chunk;
       };
-      auto publish = [&]() {
-        const int slot = sit & (kSched - 1);
-        mbar_wait(&sch_empty[slot], ((sit / kSched) & 1) ^ 1);
-        sch_tile[slot] = t;
-        mbar_arrive(&sch_full[slot]);
-        ++sit;
-      };
-      if (p.mode == 3) {
-        // halo-reuse 3x3 conv: weights are loaded once and stay resident; every tile needs ONE halo'd input tile
-        if (t < total_tiles) {
-          mbar_arrive_expect_tx(bst_bar, 9u * (uint32_t)p.bn * 128u);
-          for (int tap = 0; tap < 9; ++tap) tma_load_2d(bstat + tap * p.bn * 128, &tmB, bst_bar, tap * 64, 0);
+      for (;;) {
+        {
+          const int slot = sit & (kSched - 1);
+          mbar_wait(&sch_empty[slot], ((sit / kSched) & 1) ^ 1);
+          sch_tile[slot] = t;
+          mbar_arrive(&sch_full[slot]);
+          ++sit;
         }
-        for (;;) {
-          publish();
-          if (t >= total_tiles) {
-            if (++ends == 2) break;
-            continue;
-          }
-          // the next index is requested now and needed only after this tile's loads are queued
-          const int t_next = next_after(t);
-          const int tn = fdiv(t, p.d_twh);
-          const int r_wh = t - tn * (p.tiles_w * p.tiles_h);
-          const int th = fdiv(r_wh, p.d_tw);
-          const int tw = r_wh - th * p.tiles_w;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)(p.halo_w * kHaloH * 128));
-          tma_load_4d(smem + stage * p.stage_bytes, &tmA, &full_bar[stage], 0, (tw << 3) - 1, (th << 4) - 1, tn);
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-          t = t_next;
-        }
-      }
-      if (p.mode == 4) {
-        // halo-reuse 3x3 wgrad (64 -> 64 channels): every spatial tile of 8 x 16 positions needs ONE halo'd input tile
-        // and ONE output-gradient tile; all nine taps are row-shifted views of the halo tile
-        const uint32_t halo_bytes = (uint32_t)(p.halo_w * kHaloH * 128);
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-          const int tn = fdiv(t, p.d_twh);
-          const int r_wh = t - tn * (p.tiles_w * p.tiles_h);
-          const int th = fdiv(r_wh, p.d_tw);
-          const int tw = r_wh - th * p.tiles_w;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sX = smem + stage * p.stage_bytes;
-          mbar_arrive_expect_tx(&full_bar[stage], halo_bytes + 16384u);
-          tma_load_4d(sX, &tmB, &full_bar[stage], 0, (tw << 3) - 1, (th << 4) - 1, tn);        // x halo tile
-          tma_load_4d(sX + p.dy_off, &tmA, &full_bar[stage], 0, tw << 3, th << 4, tn);          // dy tile [128 pos][64]
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-        }
-      }
-      for (; p.mode < 3;) {
-        publish();
-        if (t >= total_tiles) {
-          if (++ends == 2) break;
-          continue;
-        }
+        if (t >= total_tiles) break;
+        // the next index is requested now and needed only after this tile's loads are queued
         const int t_next = next_after(t);
         int ks, mt, nt;
-        decode_tile(p, t, ks, mt, nt, rank);
+        decode_tile(p, t, ks, mt, nt);
         const int kb0 = ks * p.kb_per_split;
         const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
         int w0 = 0, h0 = 0, n0 = 0;
@@ -468,37 +319,32 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const int tw = r_wh - th * p.tiles_w;
           w0 = tw << p.lbw; h0 = th << p.lbh; n0 = tn << p.lbn;
         }
+        const int nb0 = nt * p.bn;  // first B row (column of the output)
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sA = smem + stage * p.stage_bytes;
           uint8_t* sB = sA + kABytes;
-          // MN-major A tiles are loaded as two 64-row atoms; when the second lies entirely beyond M it is not fetched
-          // (its accumulator rows are garbage, and masked by the epilogue)
-          // pair: every load of both CTAs counts on the LEADER's barrier, which expects the bytes of both (fixed: the
-          // half-A shortcut is off); B rows / atoms of this CTA's half of the column tile
-          const bool half_a = !kPair && p.a_mn && (mt * kBM + 64 >= p.M);
-          if (!kPair) mbar_arrive_expect_tx(&full_bar[stage], (half_a ? kABytes / 2 : kABytes) + b_bytes);
-          else if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2u * (kABytes + b_bytes));
-          const int nb0 = nt * p.bn + rank * bn_cta;  // first B row (column of the output) staged by this CTA
+          mbar_arrive_expect_tx(&full_bar[stage], kABytes + b_bytes);
           if (p.mode == 0) {
             if (!p.a_mn) {
-              LOAD2D(sA, &tmA, &full_bar[stage], kb * kBK, mt * kBM);
+              tma_load_2d(sA, &tmA, &full_bar[stage], kb * kBK, mt * kBM);
             } else {
-              LOAD2D(sA, &tmA, &full_bar[stage], mt * kBM, kb * kBK);
-              if (!half_a) LOAD2D(sA + 8192, &tmA, &full_bar[stage], mt * kBM + 64, kb * kBK);
+              tma_load_2d(sA, &tmA, &full_bar[stage], mt * kBM, kb * kBK);
+              tma_load_2d(sA + 8192, &tmA, &full_bar[stage], mt * kBM + 64, kb * kBK);
             }
             if (!p.b_mn) {
-              LOAD2D(sB, &tmB, &full_bar[stage], kb * kBK, nb0);
+              tma_load_2d(sB, &tmB, &full_bar[stage], kb * kBK, nb0);
             } else {
-              for (int j = 0; j < (bn_cta >> 6); ++j)
-                LOAD2D(sB + j * 8192, &tmB, &full_bar[stage], nb0 + 64 * j, kb * kBK);
+              for (int j = 0; j < (p.bn >> 6); ++j)
+                tma_load_2d(sB + j * 8192, &tmB, &full_bar[stage], nb0 + 64 * j, kb * kBK);
             }
           } else if (p.mode == 1) {
             const int tap = fdiv(kb, p.d_cpb);
             const int cb = kb - tap * p.cpb;
             const int kh = fdiv(tap, p.d_taps), kw = tap - kh * KP_TAPS_W;
-            LOAD4D(sA, &tmA, &full_bar[stage], cb * 64, p.cstride * w0 + kw - KP_PAD, p.cstride * h0 + kh - KP_PAD, n0);
-            LOAD2D(sB, &tmB, &full_bar[stage], kb * kBK, nb0);
+            tma_load_4d(sA, &tmA, &full_bar[stage], cb * 64, p.cstride * w0 + kw - KP_PAD, p.cstride * h0 + kh - KP_PAD,
+                        n0);
+            tma_load_2d(sB, &tmB, &full_bar[stage], kb * kBK, nb0);
           } else {
             // wgrad: reduction block kb is a spatial box of 64 output positions
             const int tn = fdiv(kb, p.d_twh);
@@ -506,17 +352,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int th = fdiv(r_wh, p.d_tw);
             const int tw = r_wh - th * p.tiles_w;
             const int bw0 = tw << p.lbw, bh0 = th << p.lbh, bn0 = tn << p.lbn;
-            LOAD4D(sA, &tmA, &full_bar[stage], mt * kBM, bw0, bh0, bn0);
-            if (!half_a) LOAD4D(sA + 8192, &tmA, &full_bar[stage], mt * kBM + 64, bw0, bh0, bn0);
-            for (int j = 0; j < (bn_cta >> 6); ++j) {
+            tma_load_4d(sA, &tmA, &full_bar[stage], mt * kBM, bw0, bh0, bn0);
+            tma_load_4d(sA + 8192, &tmA, &full_bar[stage], mt * kBM + 64, bw0, bh0, bn0);
+            for (int j = 0; j < (p.bn >> 6); ++j) {
               const int atom = (nb0 >> 6) + j;
               const int tap = fdiv(atom, p.d_cpb);
               const int cb = atom - tap * p.cpb;
               const int kh = fdiv(tap, p.d_taps), kw = tap - kh * KP_TAPS_W;
-              // atoms past the 9 taps are loaded fully out of bounds (zero fill) to keep the tx count fixed
+              // atoms past the last tap are loaded fully out of bounds (zero fill) to keep the tx count fixed
               const int nn = tap < KP_NTAPS ? bn0 : p.cN + 1;
-              LOAD4D(sB + j * 8192, &tmB, &full_bar[stage], cb * 64, p.cstride * bw0 + kw - KP_PAD,
-                     p.cstride * bh0 + kh - KP_PAD, nn);
+              tma_load_4d(sB + j * 8192, &tmB, &full_bar[stage], cb * 64, p.cstride * bw0 + kw - KP_PAD,
+                          p.cstride * bh0 + kh - KP_PAD, nn);
             }
           }
           if (++stage == nstages) { stage = 0; phase ^= 1; }
@@ -524,304 +370,152 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         t = t_next;
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    // The WHOLE warp walks the schedule (so stage / phase / descriptors are warp-uniform and live in uniform
-    // registers); only the tcgen05.mma / tcgen05.commit instructions themselves are issued by lane 0.  With the loop
-    // inside an `if (lane == 0)` region the compiler kept the descriptors in vector registers and needed ~10
-    // instructions (R2UR + ELECT/BRA.U.ANY loops) per MMA, which paced the 32-clk N = 64 MMAs of the halo modes.
-    // lane-0 broadcast: the TMEM base (read from shared memory, hence a vector register) becomes a value the compiler
-    // can treat as warp-uniform and feed to tcgen05.mma without a per-instruction ELECT / R2UR.BROADCAST sequence
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    {
-      const uint32_t idesc = make_idesc_bf16(p.bn, p.a_mn, p.b_mn, kPair ? 256 : 128);
-      const uint32_t a_step = p.a_mn ? 2048u : 32u;
-      const uint32_t b_step = p.b_mn ? 2048u : 32u;
-      const uint32_t a_lbo = p.a_mn ? 8192u : 16u;
-      const uint32_t b_lbo = p.b_mn ? 8192u : 16u;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      // tile index of schedule slot `it_` (warp-uniform), released to the producer once the whole warp has it
-      auto next_tile = [&](int it_) -> int {
-        const int slot = it_ & (kSched - 1);
-        mbar_wait(&sch_full[slot], (it_ / kSched) & 1);
-        const int t_ = __shfl_sync(0xffffffffu, sch_tile[slot], 0);
-        if (lane == 0) mbar_arrive(&sch_empty[slot]);
-        return t_;
-      };
-      if (p.mode == 3) {
-        const uint64_t bd0 = make_smem_desc(smem_u32(bstat), 16, 1024);  // mode 3 always runs bn = 64
-        for (;; ++it) {
-          const int t = next_tile(it);
-          if (t >= total_tiles) break;
-          if (it == 0) mbar_wait(bst_bar, 0);
-          const int as = it & 1;
-          mbar_wait(&tempty_bar[as], ((it >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_u + (uint32_t)as * 256u;
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + stage * p.stage_bytes);
-          // output row (dh, dw) of the 16 x 8 tile reads halo row (dh + kh) * kHaloW + (dw + kw): 8-row groups are
-          // contiguous, consecutive groups are one halo line apart (SBO), and the view starts at an arbitrary row of
-          // the TMA-written tile.  The 128B swizzle is a function of absolute shared-memory address bits (verified
-          // on B200: base_offset must stay 0), so row-shifted views of one tile serve all nine taps.
-          // An N = 64 MMA takes only ~32 clk, so the issuing thread must not spend more than a few instructions per
-          // MMA: both loops are fully unrolled and every descriptor is the tile's base descriptor plus a constant.
-          const uint64_t ad0 = make_smem_desc(sA, 16, (uint32_t)kHaloW * 128u);
-#pragma unroll 1
-          for (int tap = 0; tap < 9; ++tap) {
-            const uint64_t ad_t = ad0 + (uint64_t)((uint32_t)((tap / 3) * kHaloW + tap % 3) * 8u);  // rows * 128 B >> 4
-            const uint64_t bd_t = bd0 + (uint64_t)((uint32_t)tap * 512u);                            // 64 * 128 B >> 4
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k)
-              umma_bf16_ws(d_tmem, ad_t + (uint64_t)(2 * k), bd_t + (uint64_t)(2 * k), idesc, (tap | k) ? 1u : 0u);
-          }
-          umma_commit_ws(&empty_bar[stage]);
-          umma_commit_ws(&tfull_bar[as]);
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-        }
-      }
-      if (p.mode == 4) {
-        // D[(tap, cin) = 576 rows -> 5 M-tiles][cout = 64] accumulates in TMEM over ALL spatial tiles of this CTA.
-        // A = x^T views (MN-major: M = cin contiguous, K = positions): the two 64-row atoms of an M-tile are two taps,
-        // i.e. two row offsets into the same halo tile (LBO = their distance); a K step is 16 positions = 2 image lines
-        // of 8 pixels, one halo line apart (SBO).  B = dy^T (MN-major, one 64-cout atom, SBO 1024).
-        const uint32_t idesc4 = make_idesc_bf16(64, 1, 1);
-        constexpr uint32_t line = (uint32_t)kHaloW * 128u;
-        uint32_t acc0 = 0;  // the first MMA of every M-tile of this CTA's first spatial tile overwrites
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sX = smem_u32(smem + stage * p.stage_bytes);
-          const uint64_t ad0 = make_smem_desc(sX, 0, line);
-          const uint64_t bd0 = make_smem_desc(sX + (uint32_t)p.dy_off, 16, 1024);
-          // fully unrolled, constant descriptor increments (see mode 3): ~3 instructions per 32-clk MMA
-#pragma unroll 1
-          for (int j = 0; j < 5; ++j) {
-            const int t0 = 2 * j, t1 = (2 * j + 1 < 9) ? 2 * j + 1 : 2 * j;  // M-tile 4: second atom is padding
-            const uint32_t o0 = (uint32_t)((t0 / 3) * kHaloW + t0 % 3) * 128u;
-            const uint32_t o1 = (uint32_t)((t1 / 3) * kHaloW + t1 % 3) * 128u;
-            const uint32_t lbo = (o1 > o0) ? (o1 - o0) : 128u;
-            const uint64_t ad_j = ad0 + (uint64_t)(o0 >> 4) + ((uint64_t)(lbo >> 4) << 16);
-            const uint32_t d_j = tmem_u + (uint32_t)j * 64u;
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-              umma_bf16_ws(d_j, ad_j + (uint64_t)(((uint32_t)(2 * k) * line) >> 4), bd0 + (uint64_t)(k * 128), idesc4,
-                           k == 0 ? acc0 : 1u);
-          }
-          umma_commit_ws(&empty_bar[stage]);
-          acc0 = 1;
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_ws(&tfull_bar[0]);
-      }
-      for (; p.mode < 3; ++it) {
-        const int t = next_tile(it);
-        if (t >= total_tiles) break;
-        if (kPair && rank != 0) continue;  // the leader issues the pair's MMAs; this warp only keeps the index ring moving
-        const int ks = fdiv(t, p.d_mn);
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        const int as = it & 1;
-        mbar_wait(&tempty_bar[as], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_u + (uint32_t)as * 256u;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + stage * p.stage_bytes);
-          const uint32_t sB = sA + kABytes;
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            const uint64_t ad = make_smem_desc(sA + k * a_step, a_lbo, 1024);
-            const uint64_t bd = make_smem_desc(sB + k * b_step, b_lbo, 1024);
-            if (kPair) umma_bf16_pair_ws(d_tmem, ad, bd, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else umma_bf16_ws(d_tmem, ad, bd, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // pair: the commits arrive on the barrier of BOTH CTAs (each producer refills its own stage, each epilogue
-          // drains its own 128 accumulator lanes)
-          if (kPair) umma_commit_pair_ws(&empty_bar[stage]);
-          else umma_commit_ws(&empty_bar[stage]);
-          if (++stage == nstages) { stage = 0; phase ^= 1; }
-        }
-        if (kPair) umma_commit_pair_ws(&tfull_bar[as]);
-        else umma_commit_ws(&tfull_bar[as]);
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 4 && warp < 4 + p.epi_warps) {
-    // ===================================================== epilogue (p.epi_warps of the kEpiWarps warps)
-    const int ew = warp & 3;          // TMEM lane quadrant: lanes [32*ew, 32*ew+32)
-    // 64-wide tiles run TWO independent 8-warp groups on alternate tiles (group g owns accumulator stage g, staging
-    // buffer g and named barrier 1 + g): a narrow tile is two chunks of work per row behind a fixed chain of waits,
-    // barriers and fences, and two such chains in flight overlap each other's latencies.
-    const int ngrp = p.epi_groups;
-    const int epi_threads = p.epi_warps * 32 / ngrp;  // threads of one group
-    const int grp = (threadIdx.x - 128) / epi_threads;
-    const int bar_id = 1 + grp;
-    const int nhf = epi_threads >> 7;                 // column-chunk groups of 4 warps each
-    const int hf = ((warp - 4) >> 2) % nhf;           // this warp handles the 32-column chunks j = hf (mod nhf)
-    const int et = threadIdx.x - 128 - grp * epi_threads;  // 0..epi_threads-1 within the group
-    const bool staged = p.cbytes != 0;
-    const int nchunks = (p.bn + 31) >> 5;
-    // BN statistics: thread (scg, srg) owns 8 columns x st_rpt rows of every staged tile and keeps running partial sums
-    // in registers across all tiles of this CTA that share the same column block (scalar FADD / FFMA: the packed
-    // fp32x2 forms measured 5-9 % SLOWER on the 256-wide tiles in round 2, and moving the sums to the warp-level
-    // tensor path -- ones x Y and diag(Y^T x Y) with mma.sync.m16n8k16 fed by ldmatrix.trans from the staging tile, 14
-    // instructions per 16 x 32 elements -- measured 30-50 % slower per launch: 512 legacy HMMAs per tile cost more
-    // than the ~1200 scalar instructions they replace, profiles/r02g_gemm_launches.json vs r02f); they are reduced through shared memory and flushed with one atomic per column only when the column block changes (or
-    // at the end).  All 256 threads take part for the three tile widths the BN'd convs use: 64 / 128 / 256 columns =
-    // 8 / 16 / 32 column groups x 32 / 16 / 8 row groups of 4 / 8 / 16 rows (with the fixed 32 x 8 x 16 mapping a
-    // 64-wide tile kept 3/4 of the lanes idle while every warp still executed all 16 rows' instructions).
-    const int st_lg = (p.bn == 64) ? 3 : (p.bn == 128) ? 4 : 5;  // log2(column groups)
-    const int st_rgs = min(epi_threads >> st_lg, 32), st_rpt = 128 / st_rgs;  // <= 32 row groups: the flush scratch is one staging buffer
-    const int scg = et & ((1 << st_lg) - 1), srg = et >> st_lg;
-    const bool st_on = (scg * 8 < p.bn) && (srg < st_rgs);
-    float st_s[8], st_q[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) st_s[i] = st_q[i] = 0.f;
-    int st_nt = -1;
-    auto flush_stats = [&](uint8_t* scratch) {
-      // `scratch` is a staging buffer no TMA store is reading and nobody is writing (callers guarantee it)
-      float* scr = reinterpret_cast<float*>(scratch);
-      if (st_on) {
-#pragma unroll
-        for (int i = 0; i < 8; i += 2) {
-          *reinterpret_cast<float4*>(scr + (srg * p.bn + scg * 8 + i) * 2) =
-              make_float4(st_s[i], st_q[i], st_s[i + 1], st_q[i + 1]);
-          st_s[i] = st_q[i] = st_s[i + 1] = st_q[i + 1] = 0.f;
-        }
-      }
-      epi_bar(bar_id, epi_threads);
-      if (et < p.bn && st_nt * p.bn + et < p.N) {
-        float a = 0.f, b = 0.f;
-        for (int g = 0; g < st_rgs; ++g) {
-          const float2 v = *reinterpret_cast<const float2*>(scr + (g * p.bn + et) * 2);
-          a += v.x;
-          b += v.y;
-        }
-        if (kBnr) b *= __ldg(p.bnr_bnp + p.N + st_nt * p.bn + et);  // sum dz * (y - mean)  ->  sum dz * xhat
-        atomicAdd(p.stats + st_nt * p.bn + et, a);
-        atomicAdd(p.stats + p.N + st_nt * p.bn + et, b);
-      }
-      epi_bar(bar_id, epi_threads);
-    };
-    // asynchronous, coalesced TMA load of the residual tile of schedule slot `t_` into staging buffer `bi_`
-    // (called by ONE thread, only once the TMA store that last read that buffer has finished reading it)
-    auto issue_residual = [&](int t_, int bi_) {
-      int ks_, mt_, nt_;
-      decode_tile(p, t_, ks_, mt_, nt_, rank);
-      const int nb_ = nt_ * p.bn;
-      uint8_t* buf_ = cstage0 + (size_t)bi_ * p.cbytes;
-      const int slabs = (min(p.bn, p.N - nb_) + 63) >> 6;
-      mbar_arrive_expect_tx(&res_bar[bi_], (uint32_t)slabs * 16384u);
-      for (int sl = 0; sl < slabs; ++sl) {
-        if (p.mode & 1) {
-          const int tn_ = fdiv(mt_, p.d_twh);
-          const int rwh_ = mt_ - tn_ * (p.tiles_w * p.tiles_h);
-          const int th_ = fdiv(rwh_, p.d_tw), tw_ = rwh_ - th_ * p.tiles_w;
-          tma_load_4d(buf_ + sl * 16384, &tmR, &res_bar[bi_], nb_ + sl * 64, tw_ << p.lbw, th_ << p.lbh, tn_ << p.lbn);
-        } else {
-          tma_load_2d(buf_ + sl * 16384, &tmR, &res_bar[bi_], nb_ + sl * 64, mt_ * kBM);
-        }
-      }
-    };
-    int it = grp;
-    if (p.mode == 4) {
-      // one epilogue for the whole CTA: 5 M-tiles x 64 fp32 columns -> red.add into D[(tap,cin), cout]
-      if (blockIdx.x < total_tiles) {
-        mbar_wait(&tfull_bar[0], 0);
-        tc_fence_after();
-        float* D = reinterpret_cast<float*>(p.D);
-        for (int u = hf; u < 10; u += nhf) {  // 5 M-tiles x 2 chunks of 32 columns
-          const int j = u >> 1, half = u & 1;
-          float v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(j * 64 + half * 32), v);
-          tmem_ld_wait();
-          const int row = j * 128 + ew * 32 + lane;
-          if (row < p.M) {
-            float* op = D + (long long)row * p.ldd + half * 32;
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) red_add_v4(op + i, v[i], v[i + 1], v[i + 2], v[i + 3]);
-          }
-        }
-        tc_fence_before();
-      }
-    }
-    for (; p.mode != 4; it += ngrp) {
-      // schedule slot `it` belongs to this group (ring depth is even): read it, hand the slot back
-      const int slot = it & (kSched - 1);
-      mbar_wait(&sch_full[slot], (it / kSched) & 1);
-      const int t = sch_tile[slot];
-      mbar_arrive(&sch_empty[slot]);
-      if (t >= total_tiles) break;
-      int ks, mt, nt;
-      decode_tile(p, t, ks, mt, nt, rank);
-      const int as = it & 1;
-      const int n_base = nt * p.bn;
-      int tw = 0, th = 0, tn = 0;
-      if (p.mode & 1) {
-        tn = fdiv(mt, p.d_twh);
-        const int r_wh = mt - tn * (p.tiles_w * p.tiles_h);
-        th = fdiv(r_wh, p.d_tw);
-        tw = r_wh - th * p.tiles_w;
-      }
-      const int cbi = p.nbuf > 1 ? (it & 1) : 0;
-      uint8_t* cbuf = cstage0 + (size_t)cbi * p.cbytes;
-      if (staged) {
-        // (fused BN reduction over a TMA-loaded residual: every thread of the group must be done READING the previous
-        // tile in its statistics pass before the leader lets the next residual tile land in the same buffer)
-        if (kBnr && p.res_tma) epi_bar(bar_id, epi_threads);
-        // the TMA store that last read this staging buffer must have finished reading it
-        // (two groups: this leader's bulk groups are all stores from ITS buffer, so the latest one must be done.
-        // Round 2 also tried requesting the residual one full tile ahead -- it removed the wait for the residual,
-        // 25 % of the warp samples of the dgrad + shortcut GEMMs, but exposed the drain of the previous store -- and a
-        // third staging buffer, 305 vs 256 us; the two independent groups below made both moot.)
-        if (et == 0) {
-          if (p.nbuf > 1 && ngrp == 1) tma_store_wait_read<1>();
-          else tma_store_wait_read<0>();
-        }
-        // the column block changed: the sums kept in registers go out through the (now idle) staging buffer -- with a
-        // TMA-loaded residual that has to happen BEFORE the residual tile is requested into the same buffer
-        const bool new_block = p.stats != nullptr && st_nt != nt;
-        if (new_block && st_nt >= 0 && p.res_tma) {
-          epi_bar(bar_id, epi_threads);
-          flush_stats(cbuf);
-        }
-        if (et == 0) {
-          if (p.res_tma) issue_residual(t, cbi);  // requested now that this (group's) buffer is free
-          if (kBnr && p.bnr_prefetch) {
-            const int slabs = (min(p.bn, p.N - n_base) + 63) >> 6;
-            for (int sl = 0; sl < slabs; ++sl) {
-              if (p.mode & 1) tma_prefetch_l2_4d(&tmY, n_base + sl * 64, tw << p.lbw, th << p.lbh, tn << p.lbn);
-              else tma_prefetch_l2_2d(&tmY, n_base + sl * 64, mt * kBM);
-            }
-          }
-        }
-        epi_bar(bar_id, epi_threads);
-        if (new_block) {
-          if (st_nt >= 0 && !p.res_tma) flush_stats(cbuf);
-          st_nt = nt;
-        }
-      }
-      mbar_wait(&tfull_bar[as], (it >> 1) & 1);
-      tc_fence_after();
-      if (p.res_tma) {
-        const int uses = p.nbuf > 1 ? (it >> 1) : it;
-        mbar_wait(&res_bar[cbi], uses & 1);
-      }
+    return;
+  }
 
-      // ---------------- phase 1: TMEM -> registers -> fp32 epilogue math -> swizzled bf16 staging (or fp32 global)
-      const int r_in_tile = ew * 32 + lane;
-      long long grow = -1;
-      bool row_dead = false;  // mode 3: rows of a partial tile that lie outside the image must not reach the BN statistics
-      if (p.mode == 3) {
-        const int w = (tw << 3) + (r_in_tile & 7), h = (th << 4) + (r_in_tile >> 3);
-        row_dead = (w >= p.cW) || (h >= p.cH);
+  // ===================================================== MMA + epilogue (warpgroups 1 and 2)
+  setmaxnreg_inc<232>();
+  const int ct = threadIdx.x - 128;  // 0..255
+  const int wg = ct >> 7;            // this warpgroup owns rows [64 wg, 64 wg + 64) of every tile
+  const int wl = (ct >> 5) & 3;      // warp within the warpgroup: rows 16 wl .. 16 wl + 15 of those
+  const bool signal = (ct & 127) == 0;
+  constexpr int bar_id = 1, epi_threads = kEpiThreads;
+  const int et = ct;
+  const bool staged = p.cbytes != 0;
+  // BN statistics: thread (scg, srg) owns 8 columns x st_rpt rows of every staged tile and keeps running partial sums
+  // in registers across all tiles of this CTA that share the same column block; they are reduced through shared memory
+  // and flushed with one atomic per column only when the column block changes (or at the end).  64 / 128 / 256-wide
+  // tiles = 8 / 16 / 32 column groups x 32 / 16 / 8 row groups of 4 / 8 / 16 rows.
+  const int st_lg = (p.bn == 64) ? 3 : (p.bn == 128) ? 4 : 5;  // log2(column groups)
+  const int st_rgs = min(epi_threads >> st_lg, 32), st_rpt = 128 / st_rgs;  // <= 32 row groups: the flush scratch is one staging buffer
+  const int scg = et & ((1 << st_lg) - 1), srg = et >> st_lg;
+  const bool st_on = (scg * 8 < p.bn) && (srg < st_rgs);
+  float st_s[8], st_q[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) st_s[i] = st_q[i] = 0.f;
+  int st_nt = -1;
+  auto flush_stats = [&](uint8_t* scratch) {
+    // `scratch` is a staging buffer no TMA store is reading and nobody is writing (callers guarantee it)
+    float* scr = reinterpret_cast<float*>(scratch);
+    if (st_on) {
+#pragma unroll
+      for (int i = 0; i < 8; i += 2) {
+        *reinterpret_cast<float4*>(scr + (srg * p.bn + scg * 8 + i) * 2) =
+            make_float4(st_s[i], st_q[i], st_s[i + 1], st_q[i + 1]);
+        st_s[i] = st_q[i] = st_s[i + 1] = st_q[i + 1] = 0.f;
       }
+    }
+    epi_bar(bar_id, epi_threads);
+    if (et < p.bn && st_nt * p.bn + et < p.N) {
+      float a = 0.f, b = 0.f;
+      for (int g = 0; g < st_rgs; ++g) {
+        const float2 v = *reinterpret_cast<const float2*>(scr + (g * p.bn + et) * 2);
+        a += v.x;
+        b += v.y;
+      }
+      if (p.bnr) b *= __ldg(p.bnr_bnp + p.N + st_nt * p.bn + et);  // sum dz * (y - mean)  ->  sum dz * xhat
+      atomicAdd(p.stats + st_nt * p.bn + et, a);
+      atomicAdd(p.stats + p.N + st_nt * p.bn + et, b);
+    }
+    epi_bar(bar_id, epi_threads);
+  };
+  // asynchronous, coalesced TMA load of the residual tile of schedule slot `t_` into staging buffer `bi_`
+  // (called by ONE thread, only once the TMA store that last read that buffer has finished reading it)
+  auto issue_residual = [&](int t_, int bi_) {
+    int ks_, mt_, nt_;
+    decode_tile(p, t_, ks_, mt_, nt_);
+    const int nb_ = nt_ * p.bn;
+    uint8_t* buf_ = cstage0 + (size_t)bi_ * p.cbytes;
+    const int slabs = (min(p.bn, p.N - nb_) + 63) >> 6;
+    mbar_arrive_expect_tx(&res_bar[bi_], (uint32_t)slabs * 16384u);
+    for (int sl = 0; sl < slabs; ++sl) {
+      if (p.mode & 1) {
+        const int tn_ = fdiv(mt_, p.d_twh);
+        const int rwh_ = mt_ - tn_ * (p.tiles_w * p.tiles_h);
+        const int th_ = fdiv(rwh_, p.d_tw), tw_ = rwh_ - th_ * p.tiles_w;
+        tma_load_4d(buf_ + sl * 16384, &tmR, &res_bar[bi_], nb_ + sl * 64, tw_ << p.lbw, th_ << p.lbh, tn_ << p.lbn);
+      } else {
+        tma_load_2d(buf_ + sl * 16384, &tmR, &res_bar[bi_], nb_ + sl * 64, mt_ * kBM);
+      }
+    }
+  };
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  for (int it = 0;; ++it) {
+    const int slot = it & (kSched - 1);
+    mbar_wait(&sch_full[slot], (it / kSched) & 1);
+    const int t = sch_tile[slot];
+    mbar_arrive(&sch_empty[slot]);
+    if (t >= total_tiles) break;
+    int ks, mt, nt;
+    decode_tile(p, t, ks, mt, nt);
+    const int n_base = nt * p.bn;
+    int tw = 0, th = 0, tn = 0;
+    if (p.mode & 1) {
+      tn = fdiv(mt, p.d_twh);
+      const int r_wh = mt - tn * (p.tiles_w * p.tiles_h);
+      th = fdiv(r_wh, p.d_tw);
+      tw = r_wh - th * p.tiles_w;
+    }
+    const int cbi = p.nbuf > 1 ? (it & 1) : 0;
+    uint8_t* cbuf = cstage0 + (size_t)cbi * p.cbytes;
+    if (staged) {
+      // (fused BN reduction over a TMA-loaded residual: every thread must be done READING the previous tile in its
+      // statistics pass before the next residual tile lands in the same buffer)
+      if (p.bnr && p.res_tma) epi_bar(bar_id, epi_threads);
+      // the TMA store that last read this staging buffer must have finished reading it (with two buffers every tile
+      // commits one bulk group, so the one before the latest is this buffer's)
+      if (et == 0) {
+        if (p.nbuf > 1) tma_store_wait_read<1>();
+        else tma_store_wait_read<0>();
+      }
+      // the column block changed: the sums kept in registers go out through the (now idle) staging buffer -- with a
+      // TMA-loaded residual that has to happen BEFORE the residual tile is requested into the same buffer
+      const bool new_block = p.stats != nullptr && st_nt != nt;
+      if (new_block && st_nt >= 0 && p.res_tma) {
+        epi_bar(bar_id, epi_threads);
+        flush_stats(cbuf);
+      }
+      if (et == 0) {
+        if (p.res_tma) issue_residual(t, cbi);  // requested now that this buffer is free: it lands during the K loop
+        if (p.bnr && p.bnr_prefetch) {
+          const int slabs = (min(p.bn, p.N - n_base) + 63) >> 6;
+          for (int sl = 0; sl < slabs; ++sl) {
+            if (p.mode & 1) tma_prefetch_l2_4d(&tmY, n_base + sl * 64, tw << p.lbw, th << p.lbh, tn << p.lbn);
+            else tma_prefetch_l2_2d(&tmY, n_base + sl * 64, mt * kBM);
+          }
+        }
+      }
+      epi_bar(bar_id, epi_threads);
+      if (new_block) {
+        if (st_nt >= 0 && !p.res_tma) flush_stats(cbuf);
+        st_nt = nt;
+      }
+    }
+
+    // ---------------- K loop: fp32 accumulators of this warpgroup's 64 x BN block in registers
+    {
+      const int kb0 = ks * p.kb_per_split;
+      const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+      if (!p.a_mn && !p.b_mn) mma_tile<BN, 0, 0>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
+      else if (!p.a_mn) mma_tile<BN, 0, 1>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
+      else if (!p.b_mn) mma_tile<BN, 1, 0>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
+      else mma_tile<BN, 1, 1>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
+    }
+    if (p.res_tma) {
+      const int uses = p.nbuf > 1 ? (it >> 1) : it;
+      mbar_wait(&res_bar[cbi], uses & 1);
+    }
+
+    // ---------------- registers -> fp32 epilogue math -> swizzled bf16 staging (or fp32 global)
+    // wgmma accumulator layout: element 4 j + 2 h + e of thread (wl, lane) is row 16 wl + lane / 4 + 8 h of the
+    // warpgroup's block, column 8 j + 2 (lane % 4) + e
+    const int q = lane & 3;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int r_in_tile = wg * 64 + wl * 16 + (lane >> 2) + 8 * hr;
+      long long grow = -1;
       if (!staged || (p.residual != nullptr && !p.res_tma) || p.res_mask != nullptr) {
         if (p.mode & 1) {
           const int dw = r_in_tile & ((1 << p.lbw) - 1);
@@ -834,203 +528,189 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           grow = r < p.M ? (long long)r : -1;
         }
       }
-      const uint32_t t_row = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)as * 256u;
       const uint32_t srow = smem_u32(cbuf) + r_in_tile * 128;
       const int sw = r_in_tile & 7;
-      // one 32-column chunk j of this thread's row: v (fp32 accumulators) -> staging / global
-      auto do_chunk = [&](float* v, int j_) {
-        const int col0 = n_base + 32 * j_;
-        const bool full = col0 + 32 <= p.N;
-        const uint32_t sp = srow + (j_ >> 1) * 16384;
-        const int cb = (j_ & 1) * 4;
+      uint32_t mword = 0u;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n_base + 8 * j + 2 * q;
+        if (col >= p.N) continue;
+        const bool two = col + 1 < p.N;
+        float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
+        const uint32_t sa = srow + (j >> 3) * 16384 + ((((j & 7) ^ sw)) << 4) + q * 4;
+        // ReLU bit mask of the residual: bit (col % 32) of the 32-bit word (row * N + col) / 32 (N % 32 == 0, checked on
+        // the host), one load per row and 32-column chunk
+        uint32_t mb0 = 1u, mb1 = 1u;
+        if (p.res_mask != nullptr) {
+          if ((j & 3) == 0)
+            mword = grow >= 0 ? __ldg(reinterpret_cast<const uint32_t*>(p.res_mask) + ((grow * p.N + col) >> 5)) : 0u;
+          mb0 = (mword >> (col & 31)) & 1u;
+          mb1 = (mword >> ((col & 31) + 1)) & 1u;
+        }
         if (p.res_tma) {
-          // residual (+ optional ReLU bit mask: dz = dOut * [block output > 0], never materialised; one 32-bit word
-          // per row and 32-column chunk) added in packed bf16 -- host guarantees alpha == 1, no bias, no activation
-          if (p.res_mask != nullptr) {
-            const uint32_t mb = grow >= 0 ? *reinterpret_cast<const uint32_t*>(p.res_mask + (grow * p.N + col0) / 8) : 0u;
-            residual_chunk_packed<true>(v, sp, cb, sw, mb, row_dead);
+          // residual tile staged by TMA, added in packed bf16 after the accumulators are rounded (host guarantees
+          // alpha == 1, no bias, no activation); the optional mask zeroes residual elements
+          uint32_t r = lds32(sa);
+          if (p.res_mask != nullptr) r &= (mb0 ? 0x0000ffffu : 0u) | (mb1 ? 0xffff0000u : 0u);
+          sts32(sa, add_res_bf16x2(v0, v1, r));
+          continue;
+        }
+        v0 *= p.alpha;
+        v1 *= p.alpha;
+        if (p.bias != nullptr) {
+          v0 += __ldg(p.bias + col);
+          if (two) v1 += __ldg(p.bias + col + 1);
+        }
+        if (p.residual != nullptr && grow >= 0) {
+          const __nv_bfloat16* rp = p.residual + grow * p.ldr + col;
+          if (mb0) v0 += __bfloat162float(rp[0]);
+          if (two && mb1) v1 += __bfloat162float(rp[1]);
+        }
+        if (p.act == 1) {
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
+        } else if (p.act == 2) {
+          v0 = gelu_erf(v0);
+          v1 = gelu_erf(v1);
+        }
+        if (staged) {
+          sts32(sa, pack_bf16x2(v0, v1));  // columns >= N are clipped by the TMA store
+        } else if (grow >= 0) {
+          float* D = reinterpret_cast<float*>(p.D);
+          if (p.trans_d) {
+            // conv_mode 4: D[col, row]
+            float* op = D + (long long)col * p.ldd + grow;
+            atomicAdd(op, v0);
+            if (two) atomicAdd(op + p.ldd, v1);
           } else {
-            residual_chunk_packed<false>(v, sp, cb, sw, 0u, row_dead);
-          }
-        } else {
-          epi_math(v, p, grow, col0, full);
-          if (row_dead) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = 0.f;
-          }
-          if (staged) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const bf16x8 pk = pack8(v + 8 * i);
-              const uint32_t* w = reinterpret_cast<const uint32_t*>(&pk);
-              sts128(sp + (((cb + i) ^ sw) << 4), w[0], w[1], w[2], w[3]);
-            }
-          } else if (grow >= 0) {
-            epi_store_f32(v, p, grow, col0, full);
-          }
-        }
-      };
-      {
-        // one register buffer: up to four epilogue warps per scheduler hide the tcgen05.ld latency
-        float va[32];
-        for (int j = hf; j < nchunks && n_base + 32 * j < p.N; j += nhf) {
-          tmem_ld32(t_row + 32 * j, va);
-          tmem_ld_wait();
-          do_chunk(va, j);
-        }
-      }
-      tmem_ld_wait();
-      tc_fence_before();
-      // accumulator stage is free for the MMA warp (pair: the leader's, which waits for both CTAs' epilogues)
-      if (kPair) mbar_arrive_cluster(mapa_u32(&tempty_bar[as], 0));
-      else mbar_arrive(&tempty_bar[as]);
-
-      // fused BN reduction: this thread's rows / columns of the staged tile, and the loader of one batch of four rows of
-      // y (16 bytes each) and of the ReLU mask words; rows outside the output contribute nothing -- their mask word is 0
-      const int bnr_r0 = srg * st_rpt;           // first row of this thread (a multiple of 4)
-      const int bnr_col = n_base + scg * 8;
-      const bool bnr_on = kBnr && st_on && bnr_col < p.N;
-      // (element offsets fit 32 bits: the host checks M * ldy < 2^31; the four mask bytes of a batch share one register)
-      auto bnr_load = [&](int rb, uint4* yv, uint32_t& mbits) {
-        mbits = 0u;
-#pragma unroll
-        for (int r4 = 0; r4 < 4; ++r4) {
-          const int r = bnr_r0 + rb + r4;  // row of the tile
-          uint32_t off, lin = 0;
-          bool ok;
-          if (p.mode & 1) {
-            const int dw = r & ((1 << p.lbw) - 1);
-            const int dh = (r >> p.lbw) & ((1 << p.lbh) - 1);
-            const int dn = r >> (p.lbw + p.lbh);
-            const int w = (tw << p.lbw) + dw, h = (th << p.lbh) + dh, n = (tn << p.lbn) + dn;
-            ok = (w < p.vW) && (h < p.vH) && (n < p.cN);
-            off = (uint32_t)n * (uint32_t)p.bnr_sn + (uint32_t)h * (uint32_t)p.bnr_sh + (uint32_t)w * (uint32_t)p.bnr_sw;
-          } else {
-            lin = (uint32_t)(mt * kBM + r);
-            ok = lin < (uint32_t)p.M;
-            off = lin * (uint32_t)p.bnr_ldy;
-          }
-          yv[r4] = ok ? ldg128_nc(p.bnr_y + off + bnr_col) : make_uint4(0u, 0u, 0u, 0u);
-          const uint32_t mw = ok ? (kBnr == 2 ? (uint32_t)__ldg(p.bnr_mask + ((lin * (uint32_t)p.N + bnr_col) >> 3)) : 0xffu) : 0u;
-          mbits |= mw << (8 * r4);
-        }
-      };
-
-      if (staged) {
-        fence_proxy_async();  // make this thread's staging writes visible to the TMA (async proxy)
-        epi_bar(bar_id, epi_threads);
-        // ---------------- TMA store of the staged tile: one 64-column slab per instruction
-        if (et == 0) {
-          const int slabs = (min(p.bn, p.N - n_base) + 63) >> 6;
-          for (int sl = 0; sl < slabs; ++sl) {
-            if (p.mode & 1)
-              tma_store_4d(&tmD, cbuf + sl * 16384, n_base + sl * 64, tw << p.lbw, th << p.lbh, tn << p.lbn);
-            else
-              tma_store_2d(&tmD, cbuf + sl * 16384, n_base + sl * 64, mt * kBM);
-          }
-          tma_store_commit();
-        }
-        // ---------------- BN statistics of the staged (bf16-rounded) tile, accumulated in registers.
-        // Rows outside the problem are exact zeros (TMA zero fill; stats forbids bias/residual): no masking needed.
-        if (kBnr && bnr_on) {
-          const uint32_t cp = smem_u32(cbuf) + (scg >> 3) * 16384 + bnr_r0 * 128;
-          const int c8 = scg & 7;
-          // per-column BN parameters of this thread's 8 columns, re-read per tile (L1 hits) so that they do not occupy
-          // registers during the accumulator phase
-          // (y - mean per element, like the stand-alone pass: taking the mean out of the loop -- sum dz * y - mean * sum dz
-          // -- cancels catastrophically when |mean| >> std, which post-ReLU inputs with a common mode do produce)
-          float mean[8], sc[8], sh[8];
-          {
-            const float4 m0 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + bnr_col));
-            const float4 m1 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + bnr_col + 4));
-            mean[0] = m0.x; mean[1] = m0.y; mean[2] = m0.z; mean[3] = m0.w;
-            mean[4] = m1.x; mean[5] = m1.y; mean[6] = m1.z; mean[7] = m1.w;
-            if (kBnr == 1) {
-              const float4 a0 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 2 * p.N + bnr_col));
-              const float4 a1 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 2 * p.N + bnr_col + 4));
-              const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 3 * p.N + bnr_col));
-              const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 3 * p.N + bnr_col + 4));
-              sc[0] = a0.x; sc[1] = a0.y; sc[2] = a0.z; sc[3] = a0.w; sc[4] = a1.x; sc[5] = a1.y; sc[6] = a1.z; sc[7] = a1.w;
-              sh[0] = b0.x; sh[1] = b0.y; sh[2] = b0.z; sh[3] = b0.w; sh[4] = b1.x; sh[5] = b1.y; sh[6] = b1.z; sh[7] = b1.w;
-            }
-          }
-          // one batch of four rows: staged gradient x mask -> the two running sums
-          auto bnr_compute = [&](int rb, const uint4* yv, const uint32_t mbits) {
-#pragma unroll
-            for (int r4 = 0; r4 < 4; ++r4) {
-              const int r = rb + r4;
-              const uint4 raw = lds128(cp + r * 128 + ((c8 ^ ((bnr_r0 + r) & 7)) << 4));
-              float f[8], yy[8];
-              unpack8(*reinterpret_cast<const bf16x8*>(&raw), f);
-              unpack8(*reinterpret_cast<const bf16x8*>(&yv[r4]), yy);
-              if (kBnr == 1) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const bool on = (yy[i] * sc[i] + sh[i] > 0.f) && ((mbits >> (8 * r4)) & 0xffu) != 0u;
-                  const float dz = on ? f[i] : 0.f;
-                  st_s[i] += dz;
-                  st_q[i] += dz * (yy[i] - mean[i]);
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float dz = ((mbits >> (8 * r4 + i)) & 1u) ? f[i] : 0.f;
-                  st_s[i] += dz;
-                  st_q[i] += dz * (yy[i] - mean[i]);
-                }
-              }
-            }
-          };
-          // (A software pipeline over the row batches -- loads of batch b + 1 in flight while batch b is reduced, first
-          // batch requested before the barrier -- spilled ~60 registers at the kernel's 96-register budget and measured
-          // 0.6 ms/step SLOWER than this plain loop: profiles/r02p_*.)
-          uint4 ya[4];
-          uint32_t ma = 0u;
-          for (int rb = 0; rb < st_rpt; rb += 4) {
-            bnr_load(rb, ya, ma);
-            bnr_compute(rb, ya, ma);
-          }
-        }
-        if (!kBnr && p.stats != nullptr && st_on) {
-          const int r0 = srg * st_rpt;  // first row of this thread (a multiple of 4)
-          const uint32_t cp = smem_u32(cbuf) + (scg >> 3) * 16384 + r0 * 128;
-          const int c8 = scg & 7;
-          for (int rb = 0; rb < st_rpt; rb += 4) {
-#pragma unroll
-            for (int r4 = 0; r4 < 4; ++r4) {
-              const int r = rb + r4;
-              const uint4 raw = lds128(cp + r * 128 + ((c8 ^ ((r0 + r) & 7)) << 4));
-              float f[8];
-              unpack8(*reinterpret_cast<const bf16x8*>(&raw), f);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                st_s[i] += f[i];
-                st_q[i] += f[i] * f[i];
-              }
+            float* op = D + grow * p.ldd + col;
+            if (p.atomic) {
+              if (two) red_add_v2(op, v0, v1);
+              else atomicAdd(op, v0);
+            } else if (two) {
+              *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+            } else {
+              op[0] = v0;
             }
           }
         }
       }
     }
+
+    // fused BN reduction: this thread's rows / columns of the staged tile, and the loader of one batch of four rows of
+    // y (16 bytes each) and of the ReLU mask words; rows outside the output contribute nothing -- their mask word is 0
+    const int bnr_r0 = srg * st_rpt;           // first row of this thread (a multiple of 4)
+    const int bnr_col = n_base + scg * 8;
+    const bool bnr_on = p.bnr && st_on && bnr_col < p.N;
+    // (element offsets fit 32 bits: the host checks M * ldy < 2^31; the four mask bytes of a batch share one register)
+    auto bnr_load = [&](int rb, uint4* yv, uint32_t& mbits) {
+      mbits = 0u;
+#pragma unroll
+      for (int r4 = 0; r4 < 4; ++r4) {
+        const int r = bnr_r0 + rb + r4;  // row of the tile
+        uint32_t off, lin = 0;
+        bool ok;
+        if (p.mode & 1) {
+          const int dw = r & ((1 << p.lbw) - 1);
+          const int dh = (r >> p.lbw) & ((1 << p.lbh) - 1);
+          const int dn = r >> (p.lbw + p.lbh);
+          const int w = (tw << p.lbw) + dw, h = (th << p.lbh) + dh, n = (tn << p.lbn) + dn;
+          ok = (w < p.vW) && (h < p.vH) && (n < p.cN);
+          off = (uint32_t)n * (uint32_t)p.bnr_sn + (uint32_t)h * (uint32_t)p.bnr_sh + (uint32_t)w * (uint32_t)p.bnr_sw;
+        } else {
+          lin = (uint32_t)(mt * kBM + r);
+          ok = lin < (uint32_t)p.M;
+          off = lin * (uint32_t)p.bnr_ldy;
+        }
+        yv[r4] = ok ? ldg128_nc(p.bnr_y + off + bnr_col) : make_uint4(0u, 0u, 0u, 0u);
+        const uint32_t mw = ok ? (p.bnr == 2 ? (uint32_t)__ldg(p.bnr_mask + ((lin * (uint32_t)p.N + bnr_col) >> 3)) : 0xffu) : 0u;
+        mbits |= mw << (8 * r4);
+      }
+    };
+
     if (staged) {
-      if (et == 0) tma_store_wait_read<0>();
+      fence_proxy_async();  // make this thread's staging writes visible to the TMA (async proxy)
       epi_bar(bar_id, epi_threads);
-      if (p.stats != nullptr && st_nt >= 0) flush_stats(cstage0 + (size_t)grp * p.cbytes);
+      // ---------------- TMA store of the staged tile: one 64-column slab per instruction
+      if (et == 0) {
+        const int slabs = (min(p.bn, p.N - n_base) + 63) >> 6;
+        for (int sl = 0; sl < slabs; ++sl) {
+          if (p.mode & 1)
+            tma_store_4d(&tmD, cbuf + sl * 16384, n_base + sl * 64, tw << p.lbw, th << p.lbh, tn << p.lbn);
+          else
+            tma_store_2d(&tmD, cbuf + sl * 16384, n_base + sl * 64, mt * kBM);
+        }
+        tma_store_commit();
+      }
+      // ---------------- BN statistics of the staged (bf16-rounded) tile, accumulated in registers.
+      // Rows outside the problem are exact zeros (TMA zero fill; stats forbids bias/residual): no masking needed.
+      if (bnr_on) {
+        const uint32_t cp = smem_u32(cbuf) + (scg >> 3) * 16384 + bnr_r0 * 128;
+        const int c8 = scg & 7;
+        // (y - mean per element, like the stand-alone pass: taking the mean out of the loop -- sum dz * y - mean * sum dz
+        // -- cancels catastrophically when |mean| >> std, which post-ReLU inputs with a common mode do produce)
+        float mean[8], sc[8], sh[8];
+        {
+          const float4 m0 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + bnr_col));
+          const float4 m1 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + bnr_col + 4));
+          mean[0] = m0.x; mean[1] = m0.y; mean[2] = m0.z; mean[3] = m0.w;
+          mean[4] = m1.x; mean[5] = m1.y; mean[6] = m1.z; mean[7] = m1.w;
+          const float4 a0 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 2 * p.N + bnr_col));
+          const float4 a1 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 2 * p.N + bnr_col + 4));
+          const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 3 * p.N + bnr_col));
+          const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bnr_bnp + 3 * p.N + bnr_col + 4));
+          sc[0] = a0.x; sc[1] = a0.y; sc[2] = a0.z; sc[3] = a0.w; sc[4] = a1.x; sc[5] = a1.y; sc[6] = a1.z; sc[7] = a1.w;
+          sh[0] = b0.x; sh[1] = b0.y; sh[2] = b0.z; sh[3] = b0.w; sh[4] = b1.x; sh[5] = b1.y; sh[6] = b1.z; sh[7] = b1.w;
+        }
+        for (int rb = 0; rb < st_rpt; rb += 4) {
+          uint4 yv[4];
+          uint32_t mbits;
+          bnr_load(rb, yv, mbits);
+#pragma unroll
+          for (int r4 = 0; r4 < 4; ++r4) {
+            const int r = rb + r4;
+            const uint4 raw = lds128(cp + r * 128 + ((c8 ^ ((bnr_r0 + r) & 7)) << 4));
+            float f[8], yy[8];
+            unpack8(*reinterpret_cast<const bf16x8*>(&raw), f);
+            unpack8(*reinterpret_cast<const bf16x8*>(&yv[r4]), yy);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const bool on = p.bnr == 1 ? ((yy[i] * sc[i] + sh[i] > 0.f) && ((mbits >> (8 * r4)) & 0xffu) != 0u)
+                                         : (((mbits >> (8 * r4 + i)) & 1u) != 0u);
+              const float dz = on ? f[i] : 0.f;
+              st_s[i] += dz;
+              st_q[i] += dz * (yy[i] - mean[i]);
+            }
+          }
+        }
+      }
+      if (!p.bnr && p.stats != nullptr && st_on) {
+        const int r0 = srg * st_rpt;  // first row of this thread (a multiple of 4)
+        const uint32_t cp = smem_u32(cbuf) + (scg >> 3) * 16384 + r0 * 128;
+        const int c8 = scg & 7;
+        for (int rb = 0; rb < st_rpt; rb += 4) {
+#pragma unroll
+          for (int r4 = 0; r4 < 4; ++r4) {
+            const int r = rb + r4;
+            const uint4 raw = lds128(cp + r * 128 + ((c8 ^ ((r0 + r) & 7)) << 4));
+            float f[8];
+            unpack8(*reinterpret_cast<const bf16x8*>(&raw), f);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              st_s[i] += f[i];
+              st_q[i] += f[i] * f[i];
+            }
+          }
+        }
+      }
     }
   }
-
-  tc_fence_before();
-  // pair: neither CTA may leave (or free tensor memory) while the other can still signal one of its barriers
-  if (kPair) cluster_sync_all();
-  else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if (kPair) tmem_dealloc_pair(tmem_base, 512);
-    else tmem_dealloc(tmem_base, 512);
+  if (staged) {
+    if (et == 0) tma_store_wait_read<0>();
+    epi_bar(bar_id, epi_threads);
+    if (p.stats != nullptr && st_nt >= 0) flush_stats(cstage0);
   }
 }
-#undef LOAD2D
-#undef LOAD4D
 
 // ------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1149,11 +829,29 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   if (!g || !g->A || !g->B || !g->D) return set_error(VTX_EINVAL, "vtx_gemm: null pointer");
   if (g->M <= 0 || g->N <= 0 || g->K <= 0) return set_error(VTX_EINVAL, "vtx_gemm: empty problem");
   if (g->atomic && !g->out_f32) return set_error(VTX_EINVAL, "vtx_gemm: atomic accumulate needs fp32 output");
-  const int split_k = g->split_k > 1 ? g->split_k : 1;
-  if (split_k > 1 && !g->atomic) return set_error(VTX_EINVAL, "vtx_gemm: split_k > 1 needs atomic = 1");
+  if (g->split_k > 1 && !g->atomic) return set_error(VTX_EINVAL, "vtx_gemm: split_k > 1 needs atomic = 1");
   if (g->stats && (g->out_f32 || g->bias || g->residual || g->act || (g->alpha != 0.f && g->alpha != 1.f)))
     return set_error(VTX_EINVAL, "vtx_gemm: stats needs a plain bf16 output (no bias/residual/activation/alpha)");
   if (g->ldd % (g->out_f32 ? 4 : 8) != 0) return set_error(VTX_EINVAL, "vtx_gemm: ldd must keep rows 16B aligned");
+  // conv_mode 4 (D[(tap, cin), cout] of a 64 -> 64 3x3 conv) is the transpose of conv_mode 2's D[cout, (tap, cin)]: it
+  // runs as conv_mode 2 with a transposed store, split over the positions so that the three output tiles fill the GPU
+  if (g->conv_mode < 0 || g->conv_mode > 6 || g->conv_mode == 3)
+    return set_error(VTX_EINVAL, "vtx_gemm: conv_mode must be 0, 1, 2, 4, 5 or 6");
+  VtxGemm g4;
+  const bool trans_d = g->conv_mode == 4;
+  if (trans_d) {
+    if (g->conv_c != 64 || g->N != 64 || g->M != 9 * 64 || !g->out_f32 || !g->atomic)
+      return set_error(VTX_EINVAL, "vtx_gemm: conv_mode 4 needs C = Cout = 64, M = 576, fp32 atomic output");
+    g4 = *g;
+    g4.conv_mode = 2;
+    g4.M = g->N;
+    g4.N = g->M;
+    g4.split_k = vtx_num_sms() / 3;
+    g4.conv_stride = 1;
+    g4.conv_taps = 0;
+    g = &g4;
+  }
+  const int split_k = g->split_k > 1 ? g->split_k : 1;
 
   GemmKParams p;
   memset(&p, 0, sizeof(p));
@@ -1182,18 +880,17 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   p.cstride = cstride;
   const int ntaps = stem ? 4 : one_tap ? 1 : tap_grid ? p.ntaps : 9;
   if (p.mode == 1) { p.a_mn = 0; p.b_mn = 0; }
-  if (p.mode == 2 || p.mode == 4) { p.a_mn = 1; p.b_mn = 1; }
+  if (p.mode == 2) { p.a_mn = 1; p.b_mn = 1; }
   // ---- tile_n
   int bn = g->tile_n;
   if (bn == 0) {
     const int gran = p.b_mn ? 64 : 16;
     if (g->N >= 256) bn = 256;
     else bn = ((g->N + gran - 1) / gran) * gran;
-    // Heuristics from the round-2 sweep (scripts/tune_gemm.py, profiles/r02c_tune_gemm.txt):
+    // Width heuristics:
     //  * N = 1152 weight gradients (3x3, 128 channels) run 256-wide tiles even though the fifth tile is half empty:
-    //    every N-tile re-reads the dy operand, and 5 tiles beat 6 (72 vs 109 us for the implicit wgrad);
-    //  * problems with few tiles pick the width that minimises  rounds x (width + per-tile overhead): N = 512 with 98
-    //    M-tiles (layer4 at batch 256) runs 192-wide tiles -- 294 tiles = two full rounds -- instead of 196 256-wide ones;
+    //    every N-tile re-reads the dy operand;
+    //  * problems with few tiles pick the width that minimises  rounds x (width + per-tile overhead) over the SMs;
     //  * tiny problems (under ~100 tiles of 256) use 128-wide tiles to fill the machine.
     if (bn == 256 && split_k == 1) {
       const long mt = (g->M + kBM - 1) / kBM;
@@ -1215,29 +912,12 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   }
   if (bn < 16 || bn > 256 || bn % 16 != 0 || (p.b_mn && bn % 64 != 0))
     return set_error(VTX_EINVAL, "vtx_gemm: bad tile_n %d", bn);
+  // the kernel is instantiated for four wgmma widths; a narrower request runs the next one up (the extra B rows are
+  // zero-filled by the TMA unit, the extra output columns clipped by the store)
+  bn = bn <= 64 ? 64 : bn <= 128 ? 128 : bn <= 192 ? 192 : 256;
   p.bn = bn;
   p.n_tiles = (g->N + bn - 1) / bn;
-  // CTA pairs (cta_group::2) for the tensor-bound shapes: long K loops over 128- / 256-wide tiles.  Each CTA of a pair
-  // stages half of the B tile (whole 64-column atoms when B is MN-major), so the width must split accordingly.  Measured
-  // per shape class on B200 (profiles/r02o_gemm_launches_{pair,nopair}.json): K >= 1024 gains 10-19 %, the implicit 3x3
-  // weight gradients 17 %, plain weight gradients with both extents >= 1024 8-14 %; K = 256 / 512 convs over many rows
-  // (HBM-bound) LOSE 8-29 % and small-output weight gradients 7 %, so those keep one CTA per tile.  (Static schedule only.)
-  {
-    const char* pair_env = getenv("VTX_GEMM_PAIR");  // measurement / test knob, read per call: "0" = one CTA per tile,
-    const bool pair_off = pair_env != nullptr && pair_env[0] == '0';       // "2" = every eligible shape (tests)
-    const bool pair_all = pair_env != nullptr && pair_env[0] == '2';
-    const bool b_atoms = p.b_mn || p.mode == 2;
-    const bool halo_shape = p.mode == 1 && g->conv_c == 64 && g->N == 64;
-    const bool eligible = !pair_off && !sched_is_dynamic() && (g->conv_mode == 0 || g->conv_mode == 1 || g->conv_mode == 2) &&
-                          !stem && !halo_shape && bn >= 128 && bn % (b_atoms ? 128 : 32) == 0 &&
-                          (p.mode == 2 ? g->M >= 256 : (g->M >= 4 * kBM && g->K >= 4 * kBK));
-    bool wanted;
-    if (p.mode == 2) wanted = true;
-    else if (p.a_mn && p.b_mn) wanted = g->M >= 1024 && g->N >= 1024;
-    else wanted = g->K >= 1024;
-    p.pair = (eligible && (wanted || pair_all)) ? 1 : 0;
-  }
-  const int bn_cta = p.pair ? bn / 2 : bn;  // B rows per CTA (box height of the K-major B maps)
+  p.trans_d = trans_d ? 1 : 0;
   p.out_f32 = g->out_f32; p.atomic = g->atomic; p.act = g->act;
   p.alpha = g->alpha == 0.f ? 1.0f : g->alpha;
   p.D = g->D; p.ldd = g->ldd;
@@ -1266,6 +946,7 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     p.bnr_ldy = g->bnr_ldy;
     const char* pf = getenv("VTX_BNR_PREFETCH");  // measurement knob, read per call
     p.bnr_prefetch = (pf != nullptr && pf[0] == '0') ? 0 : 1;
+    p.bnr = g->bnr_mask == nullptr ? 1 : 2;
   }
 
   CUtensorMap tmA, tmB;
@@ -1284,7 +965,7 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     {
       uint64_t dims[2], str[1];
       uint32_t box[2];
-      if (!p.b_mn) { dims[0] = g->K; dims[1] = g->N; box[0] = 64; box[1] = (uint32_t)bn_cta; }
+      if (!p.b_mn) { dims[0] = g->K; dims[1] = g->N; box[0] = 64; box[1] = (uint32_t)bn; }
       else { dims[0] = g->N; dims[1] = g->K; box[0] = 64; box[1] = 64; }
       str[0] = g->ldb;
       if ((rc = make_tmap(&tmB, g->B, 2, dims, str, box)) != VTX_OK) return rc;
@@ -1296,10 +977,6 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     const int H = (Hin - 1) / cstride + 1, W = (Win - 1) / cstride + 1;
     if (C <= 0 || C % 64 != 0) return set_error(VTX_EINVAL, "vtx_gemm: implicit conv needs channels %% 64 == 0");
     p.cH = H; p.cW = W; p.cN = NI; p.cpb = C / 64;
-    // halo-reuse variant (mode 3): C = 64 -> 64 convs whose 9 weight taps (72 KB) stay resident in shared memory and
-    // whose input is fetched ONCE per 8 x 16 output tile as an 18 x 16 halo tile (instead of once per tap)
-    const bool halo = p.mode == 1 && !stem && !one_tap && !tap_grid && cstride == 1 && C == 64 && g->N == 64 && bn == 64 &&
-                      !g->out_f32 && g->residual == nullptr && getenv("VTX_GEMM_NO_HALO") == nullptr;
     // the activation operand of the implicit convs: [NI, H, W, C] NHWC; for the stem view [NI, H + 3, W + 3, 16] whose
     // "channel" extent is 4 pixels x 16 channels and whose W stride is ONE pixel (overlapping rows, legal for TMA)
     const uint64_t xdims[4] = {(uint64_t)C, (uint64_t)Win, (uint64_t)(stem ? Hin + 3 : Hin), (uint64_t)NI};
@@ -1307,47 +984,24 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
                               stem ? (uint64_t)(Hin + 3) * (Win + 3) * 16 : (uint64_t)Hin * Win * C};
     int bw, bh, bnn;
     choose_box(H, W, p.mode == 1 ? 128 : 64, &bw, &bh, &bnn);
-    if (halo) {
-      p.mode = 3; bw = 8; bh = 16; bnn = 1;
-      p.halo_w = kHaloW;
-    }
     p.lbw = ilog2(bw); p.lbh = ilog2(bh); p.lbn = ilog2(bnn);
     p.tiles_w = (W + bw - 1) / bw;
     p.tiles_h = (H + bh - 1) / bh;
     const int tiles_n = (NI + bnn - 1) / bnn;
-    if (p.mode == 4) {
-      // halo-reuse wgrad: D[9*C, Cout] (fp32, +=) ; A = dy [NI,H,W,Cout=64], B = x [NI,H,W,C=64]
-      if (C != 64 || g->N != 64 || g->M != 9 * C || !g->out_f32 || !g->atomic)
-        return set_error(VTX_EINVAL, "vtx_gemm: conv_mode 4 needs C = Cout = 64, M = 576, fp32 atomic output");
-      bw = 8; bh = 16; bnn = 1;
-      p.lbw = 3; p.lbh = 4; p.lbn = 0;
-      p.tiles_w = (W + 7) / 8;
-      p.tiles_h = (H + 15) / 16;
-      p.m_tiles = p.tiles_w * p.tiles_h * NI;  // spatial tiles: the schedule's only dimension
-      p.n_tiles = 1;
-      p.kb_total = 1;
-      p.halo_w = kHaloW;
-      uint64_t ad[4] = {64, (uint64_t)W, (uint64_t)H, (uint64_t)NI};
-      uint64_t as_[3] = {64, (uint64_t)W * 64, (uint64_t)H * W * 64};
-      uint32_t abox[4] = {64, 8, 16, 1};
-      if ((rc = make_tmap(&tmA, g->A, 4, ad, as_, abox)) != VTX_OK) return rc;
-      uint32_t xbox[4] = {64, 10, (uint32_t)kHaloH, 1};
-      if ((rc = make_tmap(&tmB, g->B, 4, ad, as_, xbox)) != VTX_OK) return rc;
-    } else if (p.mode & 1) {
+    if (p.mode == 1) {
       // A: activation [NI,H,W,C]; M = NI*H*W (tiled as boxes); K = 9*C; B: weights [N, 9*C] K-major
       if (g->M != NI * H * W || g->K != ntaps * C) return set_error(VTX_EINVAL, "vtx_gemm: conv fprop shape mismatch");
       // rows of a partial box below the image are real rows of the padded view: they would reach the BN statistics
       if (stem && g->stats && (W % bw != 0 || H % bh != 0))
         return set_error(VTX_EUNSUPPORTED, "vtx_gemm: conv_mode 5 with stats needs an output size tiled exactly by %dx%d", bw, bh);
       p.m_tiles = p.tiles_w * p.tiles_h * tiles_n;
-      p.kb_total = halo ? 1 : ntaps * p.cpb;
-      uint32_t box[4] = {64, (uint32_t)(halo ? p.halo_w : bw * cstride), (uint32_t)(halo ? kHaloH : bh * cstride),
-                         (uint32_t)bnn};
+      p.kb_total = ntaps * p.cpb;
+      uint32_t box[4] = {64, (uint32_t)(bw * cstride), (uint32_t)(bh * cstride), (uint32_t)bnn};
       const uint32_t es[4] = {1, (uint32_t)cstride, (uint32_t)cstride, 1};
       if ((rc = make_tmap(&tmA, g->A, 4, xdims, xstr, box, cstride > 1 ? es : nullptr)) != VTX_OK) return rc;
       uint64_t bd[2] = {(uint64_t)g->K, (uint64_t)g->N};
       uint64_t bs[1] = {(uint64_t)g->ldb};
-      uint32_t bb[2] = {64, (uint32_t)bn_cta};
+      uint32_t bb[2] = {64, (uint32_t)bn};
       if ((rc = make_tmap(&tmB, g->B, 2, bd, bs, bb)) != VTX_OK) return rc;
     } else {
       // wgrad: D[M = Cout, N = 9*C] += sum over positions dy[pos, Cout] * x_shift[pos, C]
@@ -1371,23 +1025,14 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   p.kb_per_split = (p.kb_total + p.k_splits - 1) / p.k_splits;
   p.k_splits = (p.kb_total + p.kb_per_split - 1) / p.kb_per_split;
 
-  // ---- shared-memory carve-up: [1 KB control][stages x (A 16 KB + B bn*128 B)][bf16 staging tile 128 x (bn*2+16) B]
-  // mode 3 stages hold one halo tile, rounded up to whole 1024-byte swizzle atoms
-  if (p.mode >= 3) p.pair = 0;
-  p.m_sched = p.pair ? (p.m_tiles + 1) / 2 : p.m_tiles;
-  p.stage_bytes = p.mode == 3 ? ((p.halo_w * kHaloH * 128 + 1023) / 1024) * 1024 : kABytes + bn_cta * kBK * 2;
-  p.dy_off = 0;
-  if (p.mode == 4) {
-    p.dy_off = ((p.halo_w * kHaloH * 128 + 1023) / 1024) * 1024;
-    p.stage_bytes = p.dy_off + 16384;
-  }
-  p.bstat_bytes = p.mode == 3 ? 9 * bn * 128 : 0;
+  // ---- shared-memory carve-up: [1 KB control][stages x (A 16 KB + B bn*128 B)][nbuf x bf16 staging tile 128 x bn]
+  p.stage_bytes = kABytes + bn * kBK * 2;
   p.cbytes = p.out_f32 ? 0 : ((bn + 63) / 64) * 16384;
   {
     // two staging buffers (the TMA store of tile i overlaps the epilogue of tile i+1) whenever the operand ring still
     // gets >= 4 stages, or holds a whole tile's K loop
     const int kb_tile = p.kb_per_split;
-    const int budget = kSmemTotal - 1024 /*alignment slack*/ - kCtrlBytes - p.bstat_bytes;
+    const int budget = kSmemTotal - 1024 /*alignment slack*/ - kCtrlBytes;
     int st = 0;
     p.nbuf = 1;
     if (p.cbytes) {
@@ -1401,8 +1046,6 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   }
   CUtensorMap tmD, tmR, tmY;
   memset(&tmY, 0, sizeof(tmY));
-  p.epi_warps = (bn >= 128 && p.mode != 4) ? kEpiWarps : 8;
-  p.epi_groups = 1;
   memset(&tmD, 0, sizeof(tmD));
   memset(&tmR, 0, sizeof(tmR));
   // the TMA-staged residual is added in packed bf16 AFTER the accumulator is rounded, which is only the documented
@@ -1410,11 +1053,6 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   p.res_tma = (p.cbytes && g->residual != nullptr && g->ldr % 8 == 0 &&
                (reinterpret_cast<uintptr_t>(g->residual) & 15) == 0 && p.alpha == 1.0f && g->bias == nullptr &&
                g->act == 0) ? 1 : 0;
-#define VTX_DUAL_EPI 2
-  if (p.mode != 4 && p.cbytes && p.nbuf == 2 && ((VTX_DUAL_EPI >= 1 && bn < 128 && !p.res_tma) || VTX_DUAL_EPI >= 2)) {
-    p.epi_groups = 2;
-    p.epi_warps = 16;
-  }
   if (p.cbytes) {
     if (p.mode & 1) {
       uint64_t dd[4] = {(uint64_t)g->N, (uint64_t)p.cW, (uint64_t)p.cH, (uint64_t)g->conv_n};
@@ -1466,33 +1104,27 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !attr_set[dev]) {
       cudaError_t e = cudaSuccess;
-      const void* kernels[6] = {(const void*)gemm_tc_kernel<0, 0>, (const void*)gemm_tc_kernel<1, 0>,
-                                (const void*)gemm_tc_kernel<2, 0>, (const void*)gemm_tc_kernel<0, 1>,
-                                (const void*)gemm_tc_kernel<1, 1>, (const void*)gemm_tc_kernel<2, 1>};
-      for (int i = 0; i < 6 && e == cudaSuccess; ++i)
+      const void* kernels[4] = {(const void*)gemm_wgmma_kernel<64>, (const void*)gemm_wgmma_kernel<128>,
+                                (const void*)gemm_wgmma_kernel<192>, (const void*)gemm_wgmma_kernel<256>};
+      for (int i = 0; i < 4 && e == cudaSuccess; ++i)
         e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
       if (e != cudaSuccess) return set_error(VTX_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       if (dev >= 0 && dev < 64) attr_set[dev] = true;
     }
   }
-  p.d_mn = make_fastdiv(p.m_sched * p.n_tiles);
+  p.d_mn = make_fastdiv(p.m_tiles * p.n_tiles);
   p.d_nt = make_fastdiv(p.n_tiles);
-  p.d_mt = make_fastdiv(p.m_sched);
+  p.d_mt = make_fastdiv(p.m_tiles);
   // BN statistics are kept in registers per column block: run over the row tiles first, so that a CTA's column block
-  // changes at most n_tiles - 1 times whatever order the tiles are handed out in (the activation operand of every conv
-  // with more than one column tile fits the L2, so the extra passes over it do not reach DRAM)
-  p.nt_major = (p.stats != nullptr && p.n_tiles > 1 && p.mode < 3) ? 1 : 0;
-  const long total = (long)p.m_sched * p.n_tiles * p.k_splits;  // schedule slots: tiles, or pairs of row tiles
+  // changes at most n_tiles - 1 times whatever order the tiles are handed out in
+  p.nt_major = (p.stats != nullptr && p.n_tiles > 1) ? 1 : 0;
+  const long total = (long)p.m_tiles * p.n_tiles * p.k_splits;
   const int sms = vtx_num_sms();
-  const int workers = p.pair ? sms / 2 : sms;
-  const int grid = (int)(total < workers ? total : workers) * (p.pair ? 2 : 1);
-  // many short tiles per CTA (64-wide layer1 / stem convs: ~170): one fetch hands out a few consecutive tiles
+  const int grid = (int)(total < sms ? total : sms);
+  // many short tiles per CTA (64-wide layer1 / stem convs): one fetch hands out a few consecutive tiles
   p.sched_chunk = total >= 32L * grid ? 4 : total >= 12L * grid ? 2 : 1;
-  p.sched = nullptr;
-  if (p.mode != 4 && !p.pair) {
-    const unsigned int fetches = (unsigned int)((total + p.sched_chunk - 1) / p.sched_chunk) + (unsigned int)grid;
-    p.sched = sched_slot(fetches, &p.sched_base);
-  }
+  const unsigned int fetches = (unsigned int)((total + p.sched_chunk - 1) / p.sched_chunk) + (unsigned int)grid;
+  p.sched = sched_slot(fetches, &p.sched_base);
   p.d_tw = make_fastdiv(p.tiles_w);
   p.d_twh = make_fastdiv(p.tiles_w * p.tiles_h);
   p.d_cpb = make_fastdiv(p.cpb);
@@ -1504,31 +1136,19 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = kSmemTotal;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
+    cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    attr[1].id = cudaLaunchAttributeClusterDimension;  // CTA pairs: 2-CTA clusters (the two SMs of one TPC)
-    attr[1].val.clusterDim.x = 2;
-    attr[1].val.clusterDim.y = 1;
-    attr[1].val.clusterDim.z = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = p.pair ? 2 : 1;
-    const int variant = !bnr ? 0 : (p.bnr_mask == nullptr ? 1 : 2);
+    cfg.numAttrs = 1;
     cudaError_t le;
-#define VTX_LAUNCH(B_, P_) le = cudaLaunchKernelEx(&cfg, gemm_tc_kernel<B_, P_>, tmA, tmB, tmD, tmR, tmY, p)
-    if (p.pair) {
-      if (variant == 0) VTX_LAUNCH(0, 1);
-      else if (variant == 1) VTX_LAUNCH(1, 1);
-      else VTX_LAUNCH(2, 1);
-    } else {
-      if (variant == 0) VTX_LAUNCH(0, 0);
-      else if (variant == 1) VTX_LAUNCH(1, 0);
-      else VTX_LAUNCH(2, 0);
-    }
-#undef VTX_LAUNCH
-    if (le != cudaSuccess) return set_error(VTX_ECUDA, "gemm_tc_kernel PDL launch: %s", cudaGetErrorString(le));
+    if (bn == 64) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64>, tmA, tmB, tmD, tmR, tmY, p);
+    else if (bn == 128) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128>, tmA, tmB, tmD, tmR, tmY, p);
+    else if (bn == 192) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<192>, tmA, tmB, tmD, tmR, tmY, p);
+    else le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<256>, tmA, tmB, tmD, tmR, tmY, p);
+    if (le != cudaSuccess) return set_error(VTX_ECUDA, "gemm_wgmma_kernel PDL launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(VTX_ECUDA, "gemm_tc_kernel launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error(VTX_ECUDA, "gemm_wgmma_kernel launch: %s", cudaGetErrorString(e));
   return VTX_OK;
 }

@@ -297,7 +297,7 @@ __global__ void ln_bwd_kernel(const float* __restrict__ dy_a, const __nv_bfloat1
 
 // ------------------------------------------------------------------------------- register-accumulating variants
 // Used for H in {128, 256, 512, 1024} (the generic kernels above serve every other width, e.g. H = 2048).  Same
-// arithmetic as ln_bwd_kernel / embed_bwd_kernel, different data movement (validated on B200 in round 2: -1.1 ms/step):
+// arithmetic as ln_bwd_kernel / embed_bwd_kernel, different data movement:
 //   * every lane owns the columns {lane*4 + 128*k}: the upstream gradient and z are read ONCE per row (they were read
 //     twice) and the dgamma / dbeta (/ dposition) partial sums of all rows of a warp stay in REGISTERS; the validated
 //     kernels do two shared-memory read-modify-writes per element, 4-way bank conflicted (ln_bwd) or shared-memory
@@ -494,7 +494,7 @@ embed_bwd_reg_kernel(const float* __restrict__ dy_a, const __nv_bfloat16* __rest
 // ------------------------------------------------------------------------------------------------ attention
 // One warp per (batch b, head h); head_dim = 64; Tq <= 32 queries, Tk <= 64 keys.  The five small matrix products
 // (S = Q K^T, O = P V; backward: dP = dO V^T, dQ = dS K, dK = dS^T Q, dV = P^T dO) run on mma.sync.m16n8k16 bf16
-// tiles with fp32 accumulation -- the tiles are 30x30 / 30x49, far below a tcgen05 instruction shape, and the kernel
+// tiles with fp32 accumulation -- the tiles are 30x30 / 30x49, far below a wgmma instruction shape, and the kernel
 // is bound by its q/k/v/o bytes, not by math.  Operands are staged once in shared memory (row stride 72 halves:
 // conflict-free ldmatrix); the causal + key-padding mask comes from caption_lengths and is never materialised.
 // causal == 1: key j allowed for query i iff j <= i and j < lengths[b] (captioning: future + key-padding mask);

@@ -1,5 +1,5 @@
 // The 7x7 / stride-2 / pad-3 stem convolution as a 4-tap implicit GEMM over a space-to-depth (s2d) view of the image
-// (validated on B200 in round 2; the im2col route of backbone.cu remains only for image sizes whose stem output is not
+// (the im2col route of backbone.cu remains only for image sizes whose stem output is not
 // tiled exactly by the 16 x 8 TMA boxes).
 //
 //   S[n, i, j, (r*2+q)*3 + c] = x[n, c, 2i + r - 3, 2j + q - 3]      (zero outside the image, channels 12..15 zero)

@@ -5,9 +5,9 @@
 #include <stdint.h>
 #include <string.h>
 
-// Programmatic dependent launch (validated on B200 in round 2: -0.4 ms/step).  Every kernel of the library signals at
+// Programmatic dependent launch.  Every kernel of the library signals at
 // its first instruction that dependents may be scheduled; the GEMM (the only kernel launched with the
-// programmatic-serialisation attribute) runs its prologue -- barrier init, TMEM allocation, tensor-map prefetch --
+// programmatic-serialisation attribute) runs its prologue -- barrier init, tensor-map prefetch --
 // while the previous kernel drains, then waits for it to complete and flush before its first global access.
 // Kernels launched without the attribute keep plain stream order, so nothing else changes semantics.
 #define VTX_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
@@ -52,8 +52,8 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // Counter-based RNG for dropout (masks are recomputed in backward, never stored).  One 64-bit hash (murmur3-style
-// finaliser) of (step seed, dropout site, element index / 4) serves FOUR consecutive elements, 16 bits each: the round-2
-// launch list showed the per-element hash (three 64-bit multiplies) dominating the attention and GELU kernels.
+// finaliser) of (step seed, dropout site, element index / 4) serves FOUR consecutive elements, 16 bits each: a
+// per-element hash (three 64-bit multiplies) would dominate the attention and GELU kernels.
 // Drop probability = round(p * 65536) / 65536 (p = 0.1: 0.100006), kept elements are scaled by 1 / (1 - p).
 __device__ __forceinline__ uint64_t hash_u64(uint64_t seed, uint32_t site, uint64_t ctr) {
   uint64_t x = seed ^ (0x9E3779B97F4A7C15ull * (uint64_t)(site + 1)) ^ (ctr * 0xD6E8FEB86659FD93ull);

@@ -501,7 +501,7 @@ class Engine:
             sums1 = None
             if rec["cols2"] is None:
                 if planes == 64 and stride == 1:
-                    # halo-reuse wgrad: D[(tap, cin), cout], accumulated in TMEM over all spatial tiles of a CTA
+                    # wgrad in the [(tap, cin), cout] layout (vtx_conv_w_unpack_add_t folds it into OIHW)
                     gemm(dy2, rec["a1"], dwp, 9 * planes, planes, Mout, atomic=True, lda=planes, ldb=planes, ldd=planes,
                          conv=(B, Hc, Wc, planes), conv_mode=4, out_f32=True)
                 else:
@@ -576,8 +576,8 @@ class Engine:
                 # sums (ReLU bit mask m3 of THAT block) are accumulated here, over the staged dx tiles
                 prev = blocks[bi - 1] if bi > 0 else None
                 bnr3 = None
-                # (only for the large early-layer tensors: at layer3 / layer4 sizes the longer epilogue costs what the
-                # stand-alone pass costs -- +42 us vs 44 us per launch at 50176 x 1024, profiles/r02n_*)
+                # (only for the large early-layer tensors: at layer3 / layer4 sizes the longer epilogue costs about what
+                # the stand-alone pass costs)
                 if fuse and prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
                     sums3 = self._slab_take(2 * Cin)
                     bnr3 = (prev["y3"], prev["bnp3"], sums3, prev["m3"])

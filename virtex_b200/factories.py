@@ -3,7 +3,7 @@ backbone, :344-407 textual head, :410-466 pretraining model, :503-545 optimiser,
 
 Same `PRODUCTS` names, `create` / `from_config` semantics and name mini-DSLs (`torchvision::resnet50`,
 `transdec_postnorm::L1_H1024_A16_F4096`).  Dataset / tokenizer / image-transform factories are outside the hot path
-(SURVEY.md section 2.1 #3) and are not provided; the products of the factories below run on the B200 engine.
+(SURVEY.md section 2.1 #3) and are not provided; the products of the factories below run on the H100 engine.
 """
 import re
 from functools import partial

@@ -1,4 +1,4 @@
-"""`CaptioningModel` family: drop-in for virtex/models/captioning.py:12-283 on the B200 engine.
+"""`CaptioningModel` family: drop-in for virtex/models/captioning.py:12-283 on the H100 engine.
 
 Same constructor arguments, attribute names, weight sharing between the two directions
 (captioning.py:57-63) and the same `forward(batch) -> {"loss", "loss_components", ["predictions"]}` contract.

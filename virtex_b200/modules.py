@@ -170,7 +170,7 @@ class TransformerDecoderTextualHead(TextualHead):
                  mask_future_positions: bool = True, max_caption_length: int = 30, padding_idx: int = 0):
         super().__init__(visual_feature_size, vocab_size, hidden_size)
         if hidden_size != 64 * attention_heads:
-            raise ValueError("the B200 attention kernel is specialised for head_dim 64 (A = H/64 in every VirTex config)")
+            raise ValueError("the attention kernel is specialised for head_dim 64 (A = H/64 in every VirTex config)")
         self.num_layers = num_layers
         self.attention_heads = attention_heads
         self.feedforward_size = feedforward_size

@@ -130,7 +130,7 @@ _gemm_struct = L.VtxGemm()
 def gemm(A, B, D, M, N, K, *, lda=None, ldb=None, ldd=None, a_mn=0, b_mn=0, bias=None, act=0, residual=None,
          ldr=0, stats=None, atomic=False, split_k=1, tile_n=0, conv=None, conv_mode=0, out_f32=None, residual_mask=None,
          conv_stride=1, conv_taps=0, tap_grid=None, out_view=None, d_ptr=None, bnr=None):
-    """D[M,N] = epilogue(A . B^T) through the tcgen05 kernel; see include/virtex_b200.h (VtxGemm).
+    """D[M,N] = epilogue(A . B^T) through the wgmma kernel; see include/virtex_b200.h (VtxGemm).
     bnr = (y, bnp, sums, mask or None[, y_ptr]): BN-backward reduction of the output fused into the epilogue."""
     g = _gemm_struct
     g.A, g.B, g.D = A.data_ptr(), B.data_ptr(), (D.data_ptr() if d_ptr is None else d_ptr)
@@ -175,7 +175,7 @@ def gemm(A, B, D, M, N, K, *, lda=None, ldb=None, ldd=None, a_mn=0, b_mn=0, bias
 
 
 def split_k_for(m_tiles_x_n_tiles, k_blocks, sms=None):
-    """Split-K factor for reduction-heavy (wgrad) GEMMs; thresholds from the round-2 sweep (scripts/tune_gemm.py)."""
+    """Split-K factor for reduction-heavy (wgrad) GEMMs."""
     sms = sms or num_sms()
     t = m_tiles_x_n_tiles
     if t >= sms:

@@ -1,4 +1,4 @@
-"""`Trainer.step(batch)`: the reference loop body (scripts/pretrain_virtex.py:145-163) on the B200 engine.
+"""`Trainer.step(batch)`: the reference loop body (scripts/pretrain_virtex.py:145-163) on the H100 engine.
 
     zero_grad -> forward (bf16 compute) -> backward -> [data-parallel gradient all-reduce, overlapped with backward]
     -> global-norm clip -> SGD(momentum, per-parameter lr / weight decay) -> Lookahead every k steps -> LR schedule
@@ -97,9 +97,8 @@ class Trainer:
         self._seed_base = (int(config.RANDOM_SEED) << 24) + rank * 1000003
         eng.seed.fill_(self._seed_base)
         self.comm_stream = torch.cuda.Stream(device=dev) if self.world > 1 else None
-        # (The GEMM's dynamic tile schedule -- ops.set_dynamic_gemm_schedule -- was built for the case that NCCL's CTAs
-        # hold SMs while a bucket is in flight; measured on 2 x B200 it is 0.15 ms/step SLOWER than the static schedule
-        # (23.81 vs 23.66 ms, profiles/r02n_*), so the trainer leaves the static schedule on.)
+        # (The GEMM's dynamic tile schedule -- ops.set_dynamic_gemm_schedule -- is meant for the case that NCCL's CTAs
+        # hold SMs while a bucket is in flight; the trainer leaves the static schedule on, which is the default.)
         self._pending = []
         self._ranges = self._bucket_ranges()
         if self.world > 1:  # DDP constructor semantics: rank 0's parameters and buffers everywhere
