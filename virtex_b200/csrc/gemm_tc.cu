@@ -8,14 +8,17 @@
 //                 schedule: every tile index (static round robin, or fetched from a per-launch atomic counter) is
 //                 published to the consumers through a small index ring in shared memory.  It hands most of its
 //                 registers to the consumers (setmaxnreg).
-//   warpgroups 1, 2 : MMA + epilogue, rows [0, 64) and [64, 128) of the 128-row tile: wgmma.mma_async m64nNk16
-//                 (N = tile_n in {64, 128, 192, 256}) with fp32 accumulators in registers, then bias / residual /
-//                 activation -> bf16 tile in 128B-swizzled smem -> one thread issues TMA stores (cp.async.bulk.tensor,
-//                 out-of-bounds rows/columns clipped by the hardware); a statistics pass over the staged tile
-//                 accumulates, in registers across the CTA's tiles, either the BN batch statistics of a conv output or
-//                 (p.bnr) the BN-BACKWARD sums of a gradient.  (fp32 / split-K outputs skip staging: stores or fp32
-//                 atomics straight from registers.)
-// Three mbarrier pipelines: smem full/empty (TMA <-> MMA), residual landed, and the tile-index ring.
+//   warpgroups 1, 2 : MMA + epilogue: wgmma.mma_async m64nNk16 (N = tile_n in {64, 128, 192, 256}) with fp32
+//                 accumulators in registers, then bias / residual / activation -> bf16 tile in 128B-swizzled smem ->
+//                 one thread issues TMA stores (cp.async.bulk.tensor, out-of-bounds rows/columns clipped by the
+//                 hardware); a statistics pass over the staged tile accumulates, in registers across the CTA's tiles,
+//                 either the BN batch statistics of a conv output or (p.bnr) the BN-BACKWARD sums of a gradient.
+//                 (fp32 / split-K outputs skip staging: stores or fp32 atomics straight from registers.)
+//                 Two schedules (template parameter PP, chosen per launch on the host): lockstep -- both warpgroups
+//                 on every tile, rows [0, 64) and [64, 128) -- or ping-pong -- each warpgroup computes every other
+//                 tile whole, and its epilogue overlaps the other warpgroup's MMAs (tiles up to 128 wide).
+// Mbarrier pipelines: smem full/empty (TMA <-> MMA), residual landed, the tile-index ring, and (ping-pong) the order in
+// which the two warpgroups issue their K loops.
 //
 // Operand "major-ness" is a runtime property (wgmma transpose bits + smem descriptor strides), so the same kernel serves
 // fprop (A,B K-major), dgrad (B MN-major) and wgrad (A,B MN-major) without transposing activations.
@@ -187,41 +190,48 @@ __device__ __forceinline__ void wgmma_bn(float* d, uint64_t ad, uint64_t bd, uin
   else wgmma_n256<TA, TB>(d, ad, bd, accumulate);
 }
 
-// K loop of one tile for one consumer warpgroup (rows [64 wg, 64 wg + 64) of the tile): one wgmma m64nBNk16 per 16-deep
-// K step, one commit group per stage.  A stage is handed back to the producer (one arrive per warpgroup) as soon as the
-// MMAs of the NEXT stage are issued and the ones reading it have completed, so one stage's MMAs are always in flight
-// while the warpgroup waits for the following stage.
-template <int BN, int TA, int TB>
-__device__ __forceinline__ void mma_tile(float* acc, uint8_t* smem, const GemmKParams& p, int kb0, int kb1, int wg,
-                                         uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
-                                         bool signal) {
+// K loop of one tile for one consumer warpgroup: NH wgmma m64nBNk16 per 16-deep K step (NH = 1: the 64 rows starting at
+// byte a_off of the A stage; NH = 2: all 128 rows, two MMAs sharing the B descriptor), one commit group per stage.  A
+// stage is handed back to the producer (one arrive per warpgroup) as soon as the MMAs of the NEXT stage are issued and
+// the ones reading it have completed, so one stage's MMAs are always in flight while the warpgroup waits for the
+// following stage.  `order_next` (ping-pong schedule): arrived on by every thread once the tile's last MMAs are issued,
+// which lets the other consumer warpgroup start its K loop while these complete.
+template <int BN, int NH, int TA, int TB>
+__device__ __forceinline__ void mma_tile(float* acc, uint8_t* smem, const GemmKParams& p, int kb0, int kb1,
+                                         uint32_t a_off, uint64_t* full_bar, uint64_t* empty_bar, int stage,
+                                         uint32_t phase, bool signal, uint64_t* order_next) {
   constexpr uint32_t a_step = TA ? 2048u : 32u;  // 16 k: two 8-row groups (MN-major) / 32 bytes along a row (K-major)
   constexpr uint32_t b_step = TB ? 2048u : 32u;
   constexpr uint32_t a_lbo = TA ? 8192u : 16u;
   constexpr uint32_t b_lbo = TB ? 8192u : 16u;
   int prev = -1;
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
+  for (int i = 0; i < NH * BN / 2; ++i) fence_operand(acc[i]);
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(&full_bar[stage], phase);
     const uint32_t s0 = smem_u32(smem + stage * p.stage_bytes);
-    const uint32_t sA = s0 + (uint32_t)wg * 8192u;  // 64 rows (K-major) or the wg-th 64-row atom (MN-major)
+    const uint32_t sA = s0 + a_off;  // 64 rows (K-major) or a 64-row atom (MN-major) per 8 KB
     const uint32_t sB = s0 + (uint32_t)kABytes;
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < kBK / 16; ++k)
-      wgmma_bn<BN, TA, TB>(acc, make_wgmma_desc(sA + k * a_step, a_lbo, 1024),
-                           make_wgmma_desc(sB + k * b_step, b_lbo, 1024), (kb > kb0 || k > 0) ? 1u : 0u);
+    for (int k = 0; k < kBK / 16; ++k) {
+      const uint64_t bd = make_wgmma_desc(sB + k * b_step, b_lbo, 1024);
+#pragma unroll
+      for (int h = 0; h < NH; ++h)
+        wgmma_bn<BN, TA, TB>(acc + h * (BN / 2), make_wgmma_desc(sA + h * 8192u + k * a_step, a_lbo, 1024), bd,
+                             (kb > kb0 || k > 0) ? 1u : 0u);
+    }
     wgmma_commit();
     wgmma_wait<1>();
     if (prev >= 0 && signal) mbar_arrive(&empty_bar[prev]);
     prev = stage;
     if (++stage == p.stages) { stage = 0; phase ^= 1; }
   }
+  if (order_next != nullptr) mbar_arrive(order_next);
   wgmma_wait<0>();
   if (prev >= 0 && signal) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) fence_operand(acc[i]);
+  for (int i = 0; i < NH * BN / 2; ++i) fence_operand(acc[i]);
 }
 
 // p.bnr (1: ReLU mask recomputed from y, 2: ReLU bit mask): the statistics pass over the staged output tile computes the
@@ -229,11 +239,20 @@ __device__ __forceinline__ void mma_tile(float* acc, uint8_t* smem, const GemmKP
 // output, and  sum_m dz,  sum_m dz * xhat  with dz = dA * [ReLU mask], xhat = (y - mean) * invstd  used to be a separate
 // pass over dA and y (vtx_bn_bwd_reduce).  The y tile is pulled into L2 by a TMA prefetch when the tile starts and read
 // with 16-byte loads in the pass.
-template <int BN>
+//
+// PP selects the consumer schedule:
+//   false (lockstep): both consumer warpgroups work on every tile, rows [0, 64) and [64, 128), and run its epilogue
+//         together while the tensor cores idle (BN up to 256);
+//   true (ping-pong): each consumer warpgroup computes whole 128-row tiles on its own (BN <= 128: 2 x BN / 2
+//         accumulators per thread), taking every other slot of the tile-index ring.  A pair of barriers makes the two
+//         K loops alternate whole tiles, so one warpgroup's epilogue runs while the other one's MMAs do.  Each
+//         warpgroup has its own staging buffer, residual barrier, named barrier and BN-statistics partials.
+template <int BN, bool PP>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
                   const __grid_constant__ CUtensorMap tmY, const GemmKParams p) {
+  static_assert(!PP || BN <= 128, "ping-pong tiles keep 2 x BN / 2 accumulators per thread");
   VTX_PDL_TRIGGER();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -242,8 +261,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* empty_bar = bars + kMaxStages;       // [kMaxStages]
   uint64_t* res_bar = bars + 2 * kMaxStages;     // [2] residual tile landed in staging buffer b
   uint64_t* sch_full = res_bar + 2;              // [kSched] tile index published
-  uint64_t* sch_empty = sch_full + kSched;       // [kSched] tile index read by every consumer thread
-  volatile int* sch_tile = reinterpret_cast<volatile int*>(sch_empty + kSched);  // [kSched]
+  uint64_t* sch_empty = sch_full + kSched;       // [kSched] tile index read by every consumer thread that uses it
+  uint64_t* order_bar = sch_empty + kSched;      // [2] (ping-pong) the other warpgroup has issued its tile's MMAs
+  // [kSched] tile index | (k-blocks the producer queued before the tile << 32): the latter gives the tile's first stage
+  // and phase in the operand ring (one 64-bit word: both halves are written and read together)
+  volatile unsigned long long* sch_tile = reinterpret_cast<volatile unsigned long long*>(order_bar + 2);
   uint8_t* smem = base + kCtrlBytes;                       // stage ring (1024-aligned)
   uint8_t* cstage0 = smem + p.stages * p.stage_bytes;      // bf16 staging: nbuf x [bn/64 slabs][128 rows][128 B], SW128
 
@@ -267,12 +289,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < nstages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
+      mbar_init(&empty_bar[i], PP ? 1 : 2);  // one arrive per consumer warpgroup that reads the stage
     }
-    for (int i = 0; i < 2; ++i) mbar_init(&res_bar[i], 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&res_bar[i], 1);
+      mbar_init(&order_bar[i], 128);
+    }
     for (int i = 0; i < kSched; ++i) {
       mbar_init(&sch_full[i], 1);
-      mbar_init(&sch_empty[i], kEpiThreads);
+      mbar_init(&sch_empty[i], PP ? 128 : kEpiThreads);
     }
     fence_mbar_init();
   }
@@ -286,9 +311,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const uint32_t b_bytes = (uint32_t)p.bn * kBK * 2;
       int stage = 0;
       uint32_t phase = 0;
-      // every tile index goes through the ring, whether it came from the counter or from the static schedule; one end
-      // marker (>= total_tiles) closes it
-      int t = t_first, sit = 0;
+      // every tile index goes through the ring, whether it came from the counter or from the static schedule; an end
+      // marker (>= total_tiles) closes it, published into two slots under the ping-pong schedule so that both consumer
+      // warpgroups see one
+      int t = t_first, sit = 0, kpos = 0;
       // tile after `t_`: the next one of the current chunk, else the first one of a freshly fetched chunk (dynamic), or
       // the CTA's next round-robin tile (static)
       auto next_after = [&](int t_) -> int {
@@ -296,21 +322,26 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if ((t_ + 1) % p.sched_chunk != 0 && t_ + 1 < total_tiles) return t_ + 1;
         return (int)(atomicAdd(p.sched, 1u) - p.sched_base) * p.sched_chunk;
       };
+      auto publish = [&](int t_) {
+        const int slot = sit & (kSched - 1);
+        mbar_wait(&sch_empty[slot], ((sit / kSched) & 1) ^ 1);
+        sch_tile[slot] = (unsigned long long)(uint32_t)t_ | ((unsigned long long)(uint32_t)kpos << 32);
+        mbar_arrive(&sch_full[slot]);
+        ++sit;
+      };
       for (;;) {
-        {
-          const int slot = sit & (kSched - 1);
-          mbar_wait(&sch_empty[slot], ((sit / kSched) & 1) ^ 1);
-          sch_tile[slot] = t;
-          mbar_arrive(&sch_full[slot]);
-          ++sit;
+        publish(t);
+        if (t >= total_tiles) {
+          if (PP) publish(t);
+          break;
         }
-        if (t >= total_tiles) break;
         // the next index is requested now and needed only after this tile's loads are queued
         const int t_next = next_after(t);
         int ks, mt, nt;
         decode_tile(p, t, ks, mt, nt);
         const int kb0 = ks * p.kb_per_split;
         const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+        kpos += kb1 - kb0;
         int w0 = 0, h0 = 0, n0 = 0;
         if (p.mode == 1) {
           const int tn = fdiv(mt, p.d_twh);
@@ -376,11 +407,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // ===================================================== MMA + epilogue (warpgroups 1 and 2)
   setmaxnreg_inc<232>();
   const int ct = threadIdx.x - 128;  // 0..255
-  const int wg = ct >> 7;            // this warpgroup owns rows [64 wg, 64 wg + 64) of every tile
-  const int wl = (ct >> 5) & 3;      // warp within the warpgroup: rows 16 wl .. 16 wl + 15 of those
+  const int wg = ct >> 7;            // lockstep: this warpgroup owns rows [64 wg, 64 wg + 64) of every tile
+  const int wl = (ct >> 5) & 3;      // warp within the warpgroup: rows 16 wl .. 16 wl + 15 of each 64-row block
   const bool signal = (ct & 127) == 0;
-  constexpr int bar_id = 1, epi_threads = kEpiThreads;
-  const int et = ct;
+  // the threads that share an epilogue: both warpgroups (lockstep) or one (ping-pong, named barrier 1 + wg)
+  constexpr int NH = PP ? 2 : 1;     // 64-row accumulator blocks per thread
+  constexpr int epi_threads = PP ? 128 : kEpiThreads;
+  const int bar_id = PP ? 1 + wg : 1;
+  const int et = PP ? (ct & 127) : ct;
   const bool staged = p.cbytes != 0;
   // BN statistics: thread (scg, srg) owns 8 columns x st_rpt rows of every staged tile and keeps running partial sums
   // in registers across all tiles of this CTA that share the same column block; they are reduced through shared memory
@@ -439,13 +473,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
   };
-  int stage = 0;
-  uint32_t phase = 0;
-  float acc[BN / 2];
+  float acc[NH * BN / 2];
+  // it: this warpgroup's tiles so far; sit: their ring slot (ping-pong: warpgroup wg takes slots wg, wg + 2, ...)
   for (int it = 0;; ++it) {
-    const int slot = it & (kSched - 1);
-    mbar_wait(&sch_full[slot], (it / kSched) & 1);
-    const int t = sch_tile[slot];
+    const int sit = PP ? 2 * it + wg : it;
+    const int slot = sit & (kSched - 1);
+    mbar_wait(&sch_full[slot], (sit / kSched) & 1);
+    const unsigned long long tk = sch_tile[slot];
+    const int t = (int)(uint32_t)tk;
+    const int kpos = (int)(tk >> 32);
     mbar_arrive(&sch_empty[slot]);
     if (t >= total_tiles) break;
     int ks, mt, nt;
@@ -458,7 +494,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       th = fdiv(r_wh, p.d_tw);
       tw = r_wh - th * p.tiles_w;
     }
-    const int cbi = p.nbuf > 1 ? (it & 1) : 0;
+    const int cbi = PP ? wg : p.nbuf > 1 ? (it & 1) : 0;
     uint8_t* cbuf = cstage0 + (size_t)cbi * p.cbytes;
     if (staged) {
       // (fused BN reduction over a TMA-loaded residual: every thread must be done READING the previous tile in its
@@ -467,7 +503,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // the TMA store that last read this staging buffer must have finished reading it (with two buffers every tile
       // commits one bulk group, so the one before the latest is this buffer's)
       if (et == 0) {
-        if (p.nbuf > 1) tma_store_wait_read<1>();
+        if (!PP && p.nbuf > 1) tma_store_wait_read<1>();
         else tma_store_wait_read<0>();
       }
       // the column block changed: the sums kept in registers go out through the (now idle) staging buffer -- with a
@@ -494,103 +530,205 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
 
-    // ---------------- K loop: fp32 accumulators of this warpgroup's 64 x BN block in registers
+    // ---------------- K loop: fp32 accumulators of this warpgroup's (NH x 64) x BN block in registers
     {
       const int kb0 = ks * p.kb_per_split;
       const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-      if (!p.a_mn && !p.b_mn) mma_tile<BN, 0, 0>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
-      else if (!p.a_mn) mma_tile<BN, 0, 1>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
-      else if (!p.b_mn) mma_tile<BN, 1, 0>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
-      else mma_tile<BN, 1, 1>(acc, smem, p, kb0, kb1, wg, full_bar, empty_bar, stage, phase, signal);
+      // the tile's first k-block: the producer queued kpos k-blocks before it (ping-pong: the other warpgroup's too)
+      const int stage = kpos % p.stages;
+      const uint32_t phase = (uint32_t)(kpos / p.stages) & 1u;
+      const uint32_t a_off = PP ? 0u : (uint32_t)wg * 8192u;
+      uint64_t* order_next = nullptr;
+      if (PP) {
+        // the K loops alternate whole tiles: wait until the other warpgroup has issued the MMAs of the tile before
+        // this one in the ring (warpgroup 1's tile `it` follows warpgroup 0's tile `it`, warpgroup 0's tile `it`
+        // follows warpgroup 1's tile `it - 1`)
+        if (wg == 1) mbar_wait(&order_bar[1], (uint32_t)it & 1u);
+        else if (it > 0) mbar_wait(&order_bar[0], (uint32_t)(it - 1) & 1u);
+        order_next = &order_bar[wg ^ 1];
+      }
+      if (!p.a_mn && !p.b_mn)
+        mma_tile<BN, NH, 0, 0>(acc, smem, p, kb0, kb1, a_off, full_bar, empty_bar, stage, phase, signal, order_next);
+      else if (!p.a_mn)
+        mma_tile<BN, NH, 0, 1>(acc, smem, p, kb0, kb1, a_off, full_bar, empty_bar, stage, phase, signal, order_next);
+      else if (!p.b_mn)
+        mma_tile<BN, NH, 1, 0>(acc, smem, p, kb0, kb1, a_off, full_bar, empty_bar, stage, phase, signal, order_next);
+      else
+        mma_tile<BN, NH, 1, 1>(acc, smem, p, kb0, kb1, a_off, full_bar, empty_bar, stage, phase, signal, order_next);
     }
     if (p.res_tma) {
-      const int uses = p.nbuf > 1 ? (it >> 1) : it;
+      const int uses = PP ? it : p.nbuf > 1 ? (it >> 1) : it;
       mbar_wait(&res_bar[cbi], uses & 1);
     }
 
     // ---------------- registers -> fp32 epilogue math -> swizzled bf16 staging (or fp32 global)
     // wgmma accumulator layout: element 4 j + 2 h + e of thread (wl, lane) is row 16 wl + lane / 4 + 8 h of the
-    // warpgroup's block, column 8 j + 2 (lane % 4) + e
+    // 64-row block, column 8 j + 2 (lane % 4) + e
     const int q = lane & 3;
+    // The epilogue kinds run as separate loops.  One fully unrolled loop that tests every option for every element
+    // pair spans tens of KB of code per tile; with 128 accumulators per thread it ran the 1x1 convs of layer1 at a
+    // tenth of the HBM bandwidth, whichever options were set (DESIGN.md section 1).  The plain bf16 output (every conv
+    // that feeds a BatchNorm), the TMA-staged residual and the unstaged fp32 output get compact loops of their own;
+    // bias, activation and a residual read from global memory take the general loop.
+    const bool plain = staged && !p.res_tma && p.bias == nullptr && p.residual == nullptr && p.act == 0 &&
+                       p.alpha == 1.0f;
+    const bool f32_only = !staged && p.bias == nullptr && p.residual == nullptr && p.act == 0;
+    // output row of row r of the tile (-1: outside the output)
+    auto tile_row = [&](int r) -> long long {
+      if (p.mode & 1) {
+        const int dw = r & ((1 << p.lbw) - 1);
+        const int dh = (r >> p.lbw) & ((1 << p.lbh) - 1);
+        const int dn = r >> (p.lbw + p.lbh);
+        const int w = (tw << p.lbw) + dw, h = (th << p.lbh) + dh, n = (tn << p.lbn) + dn;
+        return (w < p.cW && h < p.cH && n < p.cN) ? ((long long)(n * p.cH + h) * p.cW + w) : -1;
+      }
+      const int r_ = mt * kBM + r;
+      return r_ < p.M ? (long long)r_ : -1;
+    };
+    if (plain || p.res_tma) {
 #pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-      const int r_in_tile = wg * 64 + wl * 16 + (lane >> 2) + 8 * hr;
-      long long grow = -1;
-      if (!staged || (p.residual != nullptr && !p.res_tma) || p.res_mask != nullptr) {
-        if (p.mode & 1) {
-          const int dw = r_in_tile & ((1 << p.lbw) - 1);
-          const int dh = (r_in_tile >> p.lbw) & ((1 << p.lbh) - 1);
-          const int dn = r_in_tile >> (p.lbw + p.lbh);
-          const int w = (tw << p.lbw) + dw, h = (th << p.lbh) + dh, n = (tn << p.lbn) + dn;
-          grow = (w < p.cW && h < p.cH && n < p.cN) ? ((long long)(n * p.cH + h) * p.cW + w) : -1;
+      for (int hh = 0; hh < 2 * NH; ++hh) {
+        const int hr = hh & 1;
+        const float* accb = acc + (hh >> 1) * (BN / 2);
+        const int r_in_tile = (PP ? (hh >> 1) : wg) * 64 + wl * 16 + (lane >> 2) + 8 * hr;
+        const uint32_t srow = smem_u32(cbuf) + r_in_tile * 128 + q * 4;
+        const int sw = r_in_tile & 7;
+        // (columns >= N of the staged tile are clipped by the TMA store)
+        if (plain) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+            sts32(srow + (j >> 3) * 16384 + (((j & 7) ^ sw) << 4), pack_bf16x2(accb[4 * j + 2 * hr], accb[4 * j + 2 * hr + 1]));
+        } else if (p.res_mask == nullptr) {
+          // residual tile staged by TMA, added in packed bf16 after the accumulators are rounded (host guarantees
+          // alpha == 1, no bias, no activation)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const uint32_t sa = srow + (j >> 3) * 16384 + (((j & 7) ^ sw) << 4);
+            sts32(sa, add_res_bf16x2(accb[4 * j + 2 * hr], accb[4 * j + 2 * hr + 1], lds32(sa)));
+          }
         } else {
-          const int r = mt * kBM + r_in_tile;
-          grow = r < p.M ? (long long)r : -1;
+          // the same with the residual's ReLU bit mask: bit (col % 32) of the 32-bit word (row * N + col) / 32 (N % 32
+          // == 0, checked on the host), one load per row and 32-column chunk, zeroes residual elements
+          const long long grow = tile_row(r_in_tile);
+          uint32_t mword = 0u;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = n_base + 8 * j + 2 * q;
+            if ((j & 3) == 0)
+              mword = (grow >= 0 && col < p.N)
+                          ? __ldg(reinterpret_cast<const uint32_t*>(p.res_mask) + ((grow * p.N + col) >> 5)) : 0u;
+            const uint32_t sa = srow + (j >> 3) * 16384 + (((j & 7) ^ sw) << 4);
+            const uint32_t r = lds32(sa) & ((((mword >> (col & 31)) & 1u) ? 0x0000ffffu : 0u) |
+                                            (((mword >> ((col & 31) + 1)) & 1u) ? 0xffff0000u : 0u));
+            sts32(sa, add_res_bf16x2(accb[4 * j + 2 * hr], accb[4 * j + 2 * hr + 1], r));
+          }
         }
       }
-      const uint32_t srow = smem_u32(cbuf) + r_in_tile * 128;
-      const int sw = r_in_tile & 7;
-      uint32_t mword = 0u;
+    } else if (f32_only) {
+      float* const D = reinterpret_cast<float*>(p.D);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = n_base + 8 * j + 2 * q;
-        if (col >= p.N) continue;
-        const bool two = col + 1 < p.N;
-        float v0 = acc[4 * j + 2 * hr], v1 = acc[4 * j + 2 * hr + 1];
-        const uint32_t sa = srow + (j >> 3) * 16384 + ((((j & 7) ^ sw)) << 4) + q * 4;
-        // ReLU bit mask of the residual: bit (col % 32) of the 32-bit word (row * N + col) / 32 (N % 32 == 0, checked on
-        // the host), one load per row and 32-column chunk
-        uint32_t mb0 = 1u, mb1 = 1u;
-        if (p.res_mask != nullptr) {
-          if ((j & 3) == 0)
-            mword = grow >= 0 ? __ldg(reinterpret_cast<const uint32_t*>(p.res_mask) + ((grow * p.N + col) >> 5)) : 0u;
-          mb0 = (mword >> (col & 31)) & 1u;
-          mb1 = (mword >> ((col & 31) + 1)) & 1u;
-        }
-        if (p.res_tma) {
-          // residual tile staged by TMA, added in packed bf16 after the accumulators are rounded (host guarantees
-          // alpha == 1, no bias, no activation); the optional mask zeroes residual elements
-          uint32_t r = lds32(sa);
-          if (p.res_mask != nullptr) r &= (mb0 ? 0x0000ffffu : 0u) | (mb1 ? 0xffff0000u : 0u);
-          sts32(sa, add_res_bf16x2(v0, v1, r));
-          continue;
-        }
-        v0 *= p.alpha;
-        v1 *= p.alpha;
-        if (p.bias != nullptr) {
-          v0 += __ldg(p.bias + col);
-          if (two) v1 += __ldg(p.bias + col + 1);
-        }
-        if (p.residual != nullptr && grow >= 0) {
-          const __nv_bfloat16* rp = p.residual + grow * p.ldr + col;
-          if (mb0) v0 += __bfloat162float(rp[0]);
-          if (two && mb1) v1 += __bfloat162float(rp[1]);
-        }
-        if (p.act == 1) {
-          v0 = fmaxf(v0, 0.f);
-          v1 = fmaxf(v1, 0.f);
-        } else if (p.act == 2) {
-          v0 = gelu_erf(v0);
-          v1 = gelu_erf(v1);
-        }
-        if (staged) {
-          sts32(sa, pack_bf16x2(v0, v1));  // columns >= N are clipped by the TMA store
-        } else if (grow >= 0) {
-          float* D = reinterpret_cast<float*>(p.D);
-          if (p.trans_d) {
-            // conv_mode 4: D[col, row]
+      for (int hh = 0; hh < 2 * NH; ++hh) {
+        const int hr = hh & 1;
+        const float* accb = acc + (hh >> 1) * (BN / 2);
+        const int r_in_tile = (PP ? (hh >> 1) : wg) * 64 + wl * 16 + (lane >> 2) + 8 * hr;
+        const long long grow = tile_row(r_in_tile);
+        if (grow < 0) continue;
+        if (p.trans_d) {
+          // conv_mode 4: D[col, row]
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = n_base + 8 * j + 2 * q;
+            if (col >= p.N) continue;
             float* op = D + (long long)col * p.ldd + grow;
-            atomicAdd(op, v0);
-            if (two) atomicAdd(op + p.ldd, v1);
-          } else {
+            atomicAdd(op, accb[4 * j + 2 * hr] * p.alpha);
+            if (col + 1 < p.N) atomicAdd(op + p.ldd, accb[4 * j + 2 * hr + 1] * p.alpha);
+          }
+        } else if (p.atomic) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = n_base + 8 * j + 2 * q;
+            if (col >= p.N) continue;
             float* op = D + grow * p.ldd + col;
-            if (p.atomic) {
-              if (two) red_add_v2(op, v0, v1);
-              else atomicAdd(op, v0);
-            } else if (two) {
-              *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+            const float v0 = accb[4 * j + 2 * hr] * p.alpha, v1 = accb[4 * j + 2 * hr + 1] * p.alpha;
+            if (col + 1 < p.N) red_add_v2(op, v0, v1);
+            else atomicAdd(op, v0);
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = n_base + 8 * j + 2 * q;
+            if (col >= p.N) continue;
+            float* op = D + grow * p.ldd + col;
+            const float v0 = accb[4 * j + 2 * hr] * p.alpha, v1 = accb[4 * j + 2 * hr + 1] * p.alpha;
+            if (col + 1 < p.N) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+            else op[0] = v0;
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int hh = 0; hh < 2 * NH; ++hh) {
+        const int hr = hh & 1;
+        float* const accb = acc + (hh >> 1) * (BN / 2);
+        const int r_in_tile = (PP ? (hh >> 1) : wg) * 64 + wl * 16 + (lane >> 2) + 8 * hr;
+        long long grow = -1;
+        if (!staged || p.residual != nullptr) grow = tile_row(r_in_tile);
+        const uint32_t srow = smem_u32(cbuf) + r_in_tile * 128;
+        const int sw = r_in_tile & 7;
+        uint32_t mword = 0u;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n_base + 8 * j + 2 * q;
+          if (col >= p.N) continue;
+          const bool two = col + 1 < p.N;
+          float v0 = accb[4 * j + 2 * hr], v1 = accb[4 * j + 2 * hr + 1];
+          const uint32_t sa = srow + (j >> 3) * 16384 + ((((j & 7) ^ sw)) << 4) + q * 4;
+          // ReLU bit mask of the residual: bit (col % 32) of the 32-bit word (row * N + col) / 32 (N % 32 == 0, checked on
+          // the host), one load per row and 32-column chunk
+          uint32_t mb0 = 1u, mb1 = 1u;
+          if (p.res_mask != nullptr) {
+            if ((j & 3) == 0)
+              mword = grow >= 0 ? __ldg(reinterpret_cast<const uint32_t*>(p.res_mask) + ((grow * p.N + col) >> 5)) : 0u;
+            mb0 = (mword >> (col & 31)) & 1u;
+            mb1 = (mword >> ((col & 31) + 1)) & 1u;
+          }
+          v0 *= p.alpha;
+          v1 *= p.alpha;
+          if (p.bias != nullptr) {
+            v0 += __ldg(p.bias + col);
+            if (two) v1 += __ldg(p.bias + col + 1);
+          }
+          if (p.residual != nullptr && grow >= 0) {
+            const __nv_bfloat16* rp = p.residual + grow * p.ldr + col;
+            if (mb0) v0 += __bfloat162float(rp[0]);
+            if (two && mb1) v1 += __bfloat162float(rp[1]);
+          }
+          if (p.act == 1) {
+            v0 = fmaxf(v0, 0.f);
+            v1 = fmaxf(v1, 0.f);
+          } else if (p.act == 2) {
+            v0 = gelu_erf(v0);
+            v1 = gelu_erf(v1);
+          }
+          if (staged) {
+            sts32(sa, pack_bf16x2(v0, v1));  // columns >= N are clipped by the TMA store
+          } else if (grow >= 0) {
+            float* D = reinterpret_cast<float*>(p.D);
+            if (p.trans_d) {
+              // conv_mode 4: D[col, row]
+              float* op = D + (long long)col * p.ldd + grow;
+              atomicAdd(op, v0);
+              if (two) atomicAdd(op + p.ldd, v1);
             } else {
-              op[0] = v0;
+              float* op = D + grow * p.ldd + col;
+              if (p.atomic) {
+                if (two) red_add_v2(op, v0, v1);
+                else atomicAdd(op, v0);
+              } else if (two) {
+                *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+              } else {
+                op[0] = v0;
+              }
             }
           }
         }
@@ -708,7 +846,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (staged) {
     if (et == 0) tma_store_wait_read<0>();
     epi_bar(bar_id, epi_threads);
-    if (p.stats != nullptr && st_nt >= 0) flush_stats(cstage0);
+    if (p.stats != nullptr && st_nt >= 0) flush_stats(cstage0 + (PP ? (size_t)wg * p.cbytes : 0));
   }
 }
 
@@ -915,6 +1053,11 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   // the kernel is instantiated for four wgmma widths; a narrower request runs the next one up (the extra B rows are
   // zero-filled by the TMA unit, the extra output columns clipped by the store)
   bn = bn <= 64 ? 64 : bn <= 128 ? 128 : bn <= 192 ? 192 : 256;
+  // Ping-pong where it keeps the tile geometry: bf16 outputs whose tiles are at most 128 wide (N <= 128, or the width
+  // heuristics above chose 128).  Wider tiles would have to be split into 128-wide ones there, and the extra tiles and
+  // operand re-reads cost more than the overlap gains; fp32 / split-K outputs ran faster in lockstep as well (per-class
+  // A/B in DESIGN.md section 1).
+  const bool pingpong = bn <= 128 && !g->out_f32;
   p.bn = bn;
   p.n_tiles = (g->N + bn - 1) / bn;
   p.trans_d = trans_d ? 1 : 0;
@@ -1035,7 +1178,9 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     const int budget = kSmemTotal - 1024 /*alignment slack*/ - kCtrlBytes;
     int st = 0;
     p.nbuf = 1;
-    if (p.cbytes) {
+    if (pingpong) {
+      p.nbuf = 2;  // one staging buffer per consumer warpgroup
+    } else if (p.cbytes) {
       const int st2 = (budget - 2 * p.cbytes) / p.stage_bytes;
       if (st2 >= 4 || (st2 >= 2 && st2 >= kb_tile)) { p.nbuf = 2; st = st2; }
     }
@@ -1104,9 +1249,10 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !attr_set[dev]) {
       cudaError_t e = cudaSuccess;
-      const void* kernels[4] = {(const void*)gemm_wgmma_kernel<64>, (const void*)gemm_wgmma_kernel<128>,
-                                (const void*)gemm_wgmma_kernel<192>, (const void*)gemm_wgmma_kernel<256>};
-      for (int i = 0; i < 4 && e == cudaSuccess; ++i)
+      const void* kernels[6] = {(const void*)gemm_wgmma_kernel<64, false>,  (const void*)gemm_wgmma_kernel<128, false>,
+                                (const void*)gemm_wgmma_kernel<192, false>, (const void*)gemm_wgmma_kernel<256, false>,
+                                (const void*)gemm_wgmma_kernel<64, true>,   (const void*)gemm_wgmma_kernel<128, true>};
+      for (int i = 0; i < 6 && e == cudaSuccess; ++i)
         e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
       if (e != cudaSuccess) return set_error(VTX_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       if (dev >= 0 && dev < 64) attr_set[dev] = true;
@@ -1142,10 +1288,12 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     cudaError_t le;
-    if (bn == 64) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64>, tmA, tmB, tmD, tmR, tmY, p);
-    else if (bn == 128) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128>, tmA, tmB, tmD, tmR, tmY, p);
-    else if (bn == 192) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<192>, tmA, tmB, tmD, tmR, tmY, p);
-    else le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<256>, tmA, tmB, tmD, tmR, tmY, p);
+    if (pingpong && bn == 64) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64, true>, tmA, tmB, tmD, tmR, tmY, p);
+    else if (pingpong) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128, true>, tmA, tmB, tmD, tmR, tmY, p);
+    else if (bn == 64) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64, false>, tmA, tmB, tmD, tmR, tmY, p);
+    else if (bn == 128) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128, false>, tmA, tmB, tmD, tmR, tmY, p);
+    else if (bn == 192) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<192, false>, tmA, tmB, tmD, tmR, tmY, p);
+    else le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<256, false>, tmA, tmB, tmD, tmR, tmY, p);
     if (le != cudaSuccess) return set_error(VTX_ECUDA, "gemm_wgmma_kernel PDL launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();
