@@ -88,6 +88,7 @@ struct GemmKParams {
   void* D;
   long long ldd;
   const float* bias;
+  int bias_pairs;            // the bias can be read as float2 pairs: 8-byte aligned and N even
   const __nv_bfloat16* residual;
   long long ldr;
   const uint8_t* res_mask;   // optional bit mask [M, N/8]: the residual of (row, col) is added only where its bit is set
@@ -568,10 +569,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // The epilogue kinds run as separate loops.  One fully unrolled loop that tests every option for every element
     // pair spans tens of KB of code per tile; with 128 accumulators per thread it ran the 1x1 convs of layer1 at a
     // tenth of the HBM bandwidth, whichever options were set (DESIGN.md section 1).  The plain bf16 output (every conv
-    // that feeds a BatchNorm), the TMA-staged residual and the unstaged fp32 output get compact loops of their own;
-    // bias, activation and a residual read from global memory take the general loop.
+    // that feeds a BatchNorm), the bf16 output with a bias (the linear layers), the TMA-staged residual and the
+    // unstaged fp32 output get compact loops of their own; activation, alpha != 1, a residual read from global memory
+    // and fp32 outputs with a bias take the general loop.
     const bool plain = staged && !p.res_tma && p.bias == nullptr && p.residual == nullptr && p.act == 0 &&
                        p.alpha == 1.0f;
+    const bool bias_only = staged && p.bias_pairs && p.residual == nullptr && p.act == 0 && p.alpha == 1.0f;
     const bool f32_only = !staged && p.bias == nullptr && p.residual == nullptr && p.act == 0;
     // output row of row r of the tile (-1: outside the output)
     auto tile_row = [&](int r) -> long long {
@@ -585,7 +588,27 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int r_ = mt * kBM + r;
       return r_ < p.M ? (long long)r_ : -1;
     };
-    if (plain || p.res_tma) {
+    if (bias_only) {
+      // bf16 output + bias: fp32(acc + bias) rounded once to bf16, as the general loop computes it (alpha == 1 makes
+      // its multiplication exact, fused or not).  A thread's columns 8 j + 2 q are the same in every row it holds, so
+      // one bias pair per j serves all of them; pairs at or past N (N is even) read zeros and are clipped by the TMA
+      // store.  The swizzle (row & 7 == lane / 4) is the same for every row, which leaves one address per j.
+      // (Tested before the plain / residual branch: in that order the 256-wide instantiation spills less.)
+      const uint32_t srow = smem_u32(cbuf) + ((PP ? 0 : wg) * 64 + wl * 16 + (lane >> 2)) * 128 + q * 4;
+      const int sw = lane >> 2;
+      const int col0 = n_base + 2 * q;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = col0 + 8 * j;
+        const float2 b = col < p.N ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);
+        const uint32_t sa = srow + (j >> 3) * 16384 + (((j & 7) ^ sw) << 4);
+#pragma unroll
+        for (int hh = 0; hh < 2 * NH; ++hh) {
+          const float* accb = acc + (hh >> 1) * (BN / 2) + 4 * j + 2 * (hh & 1);
+          sts32(sa + ((hh >> 1) * 64 + 8 * (hh & 1)) * 128, pack_bf16x2(accb[0] + b.x, accb[1] + b.y));
+        }
+      }
+    } else if (plain || p.res_tma) {
 #pragma unroll
       for (int hh = 0; hh < 2 * NH; ++hh) {
         const int hr = hh & 1;
@@ -1065,6 +1088,7 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   p.alpha = g->alpha == 0.f ? 1.0f : g->alpha;
   p.D = g->D; p.ldd = g->ldd;
   p.bias = g->bias;
+  p.bias_pairs = (g->bias != nullptr && g->N % 2 == 0 && (reinterpret_cast<uintptr_t>(g->bias) & 7) == 0) ? 1 : 0;
   p.residual = reinterpret_cast<const __nv_bfloat16*>(g->residual);
   p.ldr = g->ldr;
   p.res_mask = reinterpret_cast<const uint8_t*>(g->residual_mask);
