@@ -229,6 +229,28 @@ int vtx_colsum(const void* X, int64_t ld, int M, int N, float* out, void* stream
 int vtx_argmax_rows(const float* X, int64_t ld, int M, int N, int64_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Classification pretext heads (csrc/classify.cu): LinearTextualHead's global average pool and the K-hot loss of
+ * ClassificationModel (virtex/modules/textual_heads.py:46-95, virtex/models/classification.py:43-108).  The linear layer
+ * is vtx_gemm; its bf16 logits use a leading dimension of V rounded up to 8 (the GEMM's bf16 row alignment).
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* pooled bf16 [B, C] = mean over the HW rows of each image of feat bf16 [B*HW, C] (NHWC backbone output), fp32 sums;
+   C % 8 == 0 */
+int vtx_group_mean_fwd(const void* feat, void* pooled, int B, int HW, int C, void* stream);
+/* dfeat bf16 [B*HW, C] = dpooled[b, c] / HW for every row of image b */
+int vtx_group_mean_bwd(const void* dpooled, void* dfeat, int B, int HW, int C, void* stream);
+/* Largest V the loss's shared-memory label bitmap covers; a larger V is rejected with VTX_EUNSUPPORTED. */
+#define VTX_KHOT_MAX_V 65536
+/* K-hot cross entropy over bf16 logits [B, ldl] (V valid columns) and int64 labels [B, ldlab] (L used columns).
+   U_b = distinct labels of row b in [0, V) that are not in the device array ignore[n_ignore]; labels outside [0, V)
+   are skipped, never read as a column.  loss[0] += (1/B) * (logsumexp_b - mean_{u in U_b} z[b, u]), which is NaN for
+   an empty U_b.  write_grad: logits := (softmax - [v in U_b] / |U_b|) / B in place, a zero row for an empty U_b. */
+int vtx_khot_xent(void* logits, int64_t ldl, const int64_t* labels, int64_t ldlab, int B, int L, int V,
+                  const int64_t* ignore, int n_ignore, float* loss, int write_grad, void* stream);
+/* out int64 [M, k] = column indices of the k largest values of each row of fp32 X [M, ld] (N columns), in descending
+   order; equal values in ascending index order; NaN ranks as -inf.  Needs k <= N. */
+int vtx_topk_rows(const float* X, int64_t ld, int M, int N, int k, int64_t* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * GPU input pipeline (csrc/input_pipe.cu): decoded uint8 HWC images -> fp32 NCHW network input, token lists -> padded
  * matrices.  Replaces the per-sample albumentations / cv2 transforms and the collate of
  * virtex/data/datasets/captioning.py:51-100 with the transform lists of virtex/factories.py:131-155.  Random parameters

@@ -25,6 +25,7 @@ import torch
 from torch import nn
 
 from . import ops
+from .modules import LinearTextualHead
 from .ops import call, gemm, _p, _stream
 
 BF16, F32 = torch.bfloat16, torch.float32
@@ -124,7 +125,7 @@ def _require_cuda(dev):
 class Engine:
     """Forward/backward of (backbone) + (forward head) + (backward head) on one GPU.  Any part may be absent."""
 
-    def __init__(self, visual=None, textual=None, backward_textual=None, prefix_map=None):
+    def __init__(self, visual=None, textual=None, backward_textual=None, prefix_map=None, ignore_indices=None):
         self.visual, self.textual, self.backward_textual = visual, textual, backward_textual
         named: List[Tuple[str, nn.Parameter]] = []
         if visual is not None:
@@ -145,7 +146,13 @@ class Engine:
         if visual is not None:
             self.buffers.update({"visual." + n: b for n, b in visual.named_buffers()})
         head = textual if textual is not None else backward_textual
-        self.pad = head.padding_idx if head is not None else 0
+        self.pad = getattr(head, "padding_idx", 0) if head is not None else 0
+        # a LinearTextualHead makes this the engine of a classification pretext model: pool + linear + K-hot loss instead
+        # of a decoder (virtex/models/classification.py:43-108)
+        self.classify = isinstance(textual, LinearTextualHead)
+        # label ids the K-hot loss ignores, on the device once per engine (read by every loss launch)
+        self.ignore = torch.tensor([int(i) for i in (ignore_indices or [])], dtype=torch.int64, device=dev)
+        self._cls = None
         self.seed = torch.zeros(1, dtype=torch.int64, device=dev)
         self.loss = torch.zeros(2, dtype=F32, device=dev)       # per-direction mean NLL
         self.count = torch.zeros(2, dtype=F32, device=dev)      # per-direction number of valid targets
@@ -931,6 +938,67 @@ class Engine:
              self.pad, p, seed, di * 1000, s)
         return dmem_started
 
+    # ------------------------------------------------------------------------------------------------ classification
+    def _pooled_logits(self, feat, B, hw, bf16=True, f32=False):
+        """LinearTextualHead: pooled [B, C] = mean of the hw feature rows of each image; logits = pooled . W^T + b.
+        bf16 logits (the loss's input) and / or fp32 logits (top-k), both with a leading dimension of V rounded up to
+        8 -- the GEMM's bf16 row alignment -- so V = 81 (multilabel) runs with ld 88."""
+        C, V = feat.shape[1], self.textual.vocab_size
+        ld = _round_up(V, 8)
+        pooled = self.ws.get("cls.pooled", (B, C), BF16)
+        call("vtx_group_mean_fwd", feat.data_ptr(), pooled.data_ptr(), B, hw, C, _stream())
+        w, b = self.W("textual.output.weight"), self.P("textual.output.bias")
+        lf = logits = None
+        if f32:
+            lf = self.ws.get("cls.logits_f32", (B, ld), F32)
+            gemm(pooled, w, lf, B, V, C, bias=b)
+        if bf16:
+            logits = self.ws.get("cls.logits", (B, ld), BF16)
+            gemm(pooled, w, logits, B, V, C, bias=b)
+        return pooled, logits, lf
+
+    def classification_forward(self, feat, hw, labels, training, with_grad):
+        """K-hot cross entropy of int64 labels [B, L] (classification.py:74-96) into self.loss[0]; leaves dlogits in
+        the bf16 logits buffer when `with_grad`, fp32 logits for top-k when not `training`."""
+        B = feat.shape[0] // hw
+        V = self.textual.vocab_size
+        pooled, logits, lf = self._pooled_logits(feat, B, hw, f32=not training)
+        call("vtx_khot_xent", logits.data_ptr(), logits.stride(0), labels.data_ptr(), labels.stride(0), B,
+             labels.shape[1], V, self.ignore.data_ptr(), self.ignore.numel(), self.loss.data_ptr(), int(with_grad),
+             _stream())
+        self._cls = dict(B=B, hw=hw, pooled=pooled, logits=logits, logits_f32=lf, with_grad=with_grad)
+        self._feat = feat
+
+    def classification_backward(self, bucket_cb=None):
+        """Linear layer backward from the dlogits written by the loss, then the pool's adjoint into the backbone."""
+        c = self._cls
+        if c is None or not c["with_grad"]:
+            raise RuntimeError("backward needs a preceding forward with with_grad=True (it leaves dlogits behind)")
+        B, hw = c["B"], c["hw"]
+        C, V = self._feat.shape[1], self.textual.vocab_size
+        frozen = getattr(self.visual, "frozen", False)
+        dpooled = None if frozen else self.ws.get("cls.dpooled", (B, C), BF16)
+        # dgrad with K = V over the padded ld: the TMA zero-fills the K tail of both operands
+        self._linear_bwd(c["logits"], c["pooled"], "textual.output.weight", "textual.output.bias", dpooled, B, V, C)
+        if bucket_cb is not None:
+            bucket_cb("head")
+        if not frozen:
+            dfeat = self.ws.get("hb.dfeat", (B * hw, C), BF16)
+            call("vtx_group_mean_bwd", dpooled.data_ptr(), dfeat.data_ptr(), B, hw, C, _stream())
+            self.backbone_backward(dfeat, bucket_cb)
+        if bucket_cb is not None:
+            bucket_cb("rest")
+
+    def classification_topk(self, k):
+        """Indices of the k largest fp32 logits of each image of the last eval-mode forward -> int64 [B, k]."""
+        c = self._cls
+        if c is None or c["logits_f32"] is None:
+            raise RuntimeError("predictions need an eval-mode forward (model.eval()) first")
+        lf = c["logits_f32"]
+        out = self.ws.get("cls.topk", (c["B"], k), torch.int64)
+        call("vtx_topk_rows", lf.data_ptr(), lf.stride(0), c["B"], self.textual.vocab_size, k, out.data_ptr(), _stream())
+        return out
+
     # ------------------------------------------------------------------------------------------------ full model
     def forward(self, image, tokens, noitpac, lengths, training=True, with_grad=True, labels=None):
         """Loss of the bicaptioning model (labels None) or of the masked-LM sibling (labels = masked_labels [B,T], single
@@ -944,6 +1012,9 @@ class Engine:
         # frozen backbone's BN back into batch-statistics mode (visual_backbones.py:48-52 only calls .eval() once)
         bn_training = bool(self.visual.cnn.training) if self.visual is not None else training
         feat, h, w = self.backbone_forward(image, bn_training)
+        if self.classify:
+            self.classification_forward(feat, h * w, labels, training, with_grad)
+            return self.loss
         B = image.shape[0]
         S = B * h * w
         mem = self.visual_projection_forward(feat, S)
@@ -961,6 +1032,9 @@ class Engine:
         backward order) so a data-parallel all-reduce can overlap the remaining backward."""
         if zero_grads:
             self.arena.grads.zero_()
+        if self.classify:
+            self.classification_backward(bucket_cb)
+            return
         feat, mem = self._feat, self._mem
         S, H = mem.shape
         dmem = self.ws.get("hb.dmem", (S, H), BF16)
@@ -982,7 +1056,10 @@ class Engine:
             bucket_cb("rest")
 
     def predictions(self):
-        """argmax over the fp32 forward-direction logits of the last eval-mode forward -> int64 [B,T]."""
+        """argmax over the fp32 forward-direction logits of the last eval-mode forward -> int64 [B,T]; for a
+        classification head the top-10 classes of each image -> int64 [B, 10] (classification.py:104-106)."""
+        if self.classify:
+            return self.classification_topk(10)
         rec = self._recs[0]
         lf = rec["logits_f32"]
         out = self.ws.get("pred", (rec["M"],), torch.int64)
@@ -1024,3 +1101,15 @@ def head_logits(head, visual_features, caption_tokens, caption_lengths) -> torch
     rec = eng.head_forward("textual", mem, caption_tokens.contiguous(), caption_lengths.contiguous(),
                            training=head.training, want_logits_f32=True)
     return rec["logits_f32"].view(B, caption_tokens.shape[1], -1).clone()
+
+
+@torch.no_grad()
+def linear_head_logits(head, visual_features) -> torch.Tensor:
+    """`LinearTextualHead.forward`: (B,C,h,w) -> fp32 logits (B,V)."""
+    eng = _module_engine(head, textual=head)
+    eng.mark_weights_dirty()
+    eng.prepare_weights()
+    B, C, h, w = visual_features.shape
+    feat = visual_features.permute(0, 2, 3, 1).reshape(B * h * w, C).to(BF16).contiguous()
+    _, _, lf = eng._pooled_logits(feat, B, h * w, bf16=False, f32=True)
+    return lf[:, :head.vocab_size].clone()

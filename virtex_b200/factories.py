@@ -55,6 +55,15 @@ class TextualHeadFactory(Factory):
         "transdec_prenorm": partial(modules.TransformerDecoderTextualHead, norm_first=True),
         "transdec_postnorm": partial(modules.TransformerDecoderTextualHead, norm_first=False),
     }
+    # the head of the pretext tasks without language modelling (token / multilabel classification): kept apart from
+    # PRODUCTS, which lists the transformer decoders, and resolved by `create` like a product
+    LINEAR_PRODUCTS: Dict[str, Callable] = {"none": modules.LinearTextualHead}
+
+    @classmethod
+    def create(cls, name: str, *args, **kwargs) -> Any:
+        if name in cls.LINEAR_PRODUCTS:
+            return cls.LINEAR_PRODUCTS[name](*args, **kwargs)
+        return super().create(name, *args, **kwargs)
 
     @classmethod
     def from_config(cls, config: Config) -> nn.Module:
@@ -105,6 +114,8 @@ class PretrainingModelFactory(Factory):
         "bicaptioning": vmodels.BidirectionalCaptioningModel,
         "captioning": vmodels.ForwardCaptioningModel,
         "masked_lm": vmodels.MaskedLMModel,
+        "token_classification": vmodels.TokenClassificationModel,
+        "multilabel_classification": vmodels.MultiLabelClassificationModel,
     }
 
     @classmethod
@@ -116,6 +127,10 @@ class PretrainingModelFactory(Factory):
         if _C.MODEL.NAME in {"virtex", "captioning", "bicaptioning"}:
             kwargs = {"sos_index": _C.DATA.SOS_INDEX, "eos_index": _C.DATA.EOS_INDEX,
                       "decoder": CaptionDecoderFactory.from_config(_C)}
+        elif _C.MODEL.NAME == "token_classification":  # special tokens are no classification targets
+            kwargs = {"ignore_indices": [_C.DATA.UNK_INDEX, _C.DATA.SOS_INDEX, _C.DATA.EOS_INDEX, _C.DATA.MASK_INDEX]}
+        elif _C.MODEL.NAME == "multilabel_classification":
+            kwargs = {"ignore_indices": [0]}  # background category
         return cls.create(_C.MODEL.NAME, visual, textual, **kwargs)
 
 

@@ -8,13 +8,13 @@ The throughput path (`virtex_b200.trainer.Trainer`) drives the same engine witho
 """
 import copy
 import functools
-from typing import Any, Dict
+from typing import Any, Dict, List
 
 import torch
 from torch import nn
 
 from .engine import Engine
-from .modules import TextualHead, VisualBackbone
+from .modules import LinearTextualHead, TextualHead, VisualBackbone
 
 
 class _StepFunction(torch.autograd.Function):
@@ -58,31 +58,18 @@ class _StepFunction(torch.autograd.Function):
         return (None, None, None, None, None, None, *grads)
 
 
-class CaptioningModel(nn.Module):
-    def __init__(self, visual: VisualBackbone, textual: TextualHead, caption_backward: bool = False,
-                 sos_index: int = 1, eos_index: int = 2, decoder: Any = None):
-        super().__init__()
-        self.visual = visual
-        self.textual = textual
-        self.padding_idx = self.textual.padding_idx
-        self.caption_backward = caption_backward
-        if self.caption_backward:
-            self.backward_textual = copy.deepcopy(self.textual)
-            # share visual projection and input/output embeddings between directions (captioning.py:60-63)
-            self.backward_textual.visual_projection = self.textual.visual_projection
-            self.backward_textual.embedding = self.textual.embedding
-            self.backward_textual.output = self.textual.output
-        self.sos_index = sos_index
-        self.eos_index = eos_index
-        self.decoder = decoder
-        self._engine = None
+class _EngineModel(nn.Module):
+    """A model whose arithmetic runs on an `Engine` over its own parameters, built lazily and rebuilt after the module
+    is moved or cast (which re-points the parameters away from the engine's arena)."""
 
-    # ---------------------------------------------------------------------------------------------------- engine
+    def _new_engine(self) -> Engine:
+        raise NotImplementedError
+
     @property
     def engine(self) -> Engine:
         eng = self._engine
         if eng is None or not eng.arena.intact():
-            eng = Engine(self.visual, self.textual, self.backward_textual if self.caption_backward else None)
+            eng = self._new_engine()
             object.__setattr__(self, "_engine", eng)
             names = {}
             for n in eng.arena.names:
@@ -101,6 +88,29 @@ class CaptioningModel(nn.Module):
         if self._engine is not None:
             self._engine.mark_weights_dirty()
         return out
+
+
+class CaptioningModel(_EngineModel):
+    def __init__(self, visual: VisualBackbone, textual: TextualHead, caption_backward: bool = False,
+                 sos_index: int = 1, eos_index: int = 2, decoder: Any = None):
+        super().__init__()
+        self.visual = visual
+        self.textual = textual
+        self.padding_idx = self.textual.padding_idx
+        self.caption_backward = caption_backward
+        if self.caption_backward:
+            self.backward_textual = copy.deepcopy(self.textual)
+            # share visual projection and input/output embeddings between directions (captioning.py:60-63)
+            self.backward_textual.visual_projection = self.textual.visual_projection
+            self.backward_textual.embedding = self.textual.embedding
+            self.backward_textual.output = self.textual.output
+        self.sos_index = sos_index
+        self.eos_index = eos_index
+        self.decoder = decoder
+        self._engine = None
+
+    def _new_engine(self) -> Engine:
+        return Engine(self.visual, self.textual, self.backward_textual if self.caption_backward else None)
 
     # ---------------------------------------------------------------------------------------------------- forward
     def forward(self, batch: Dict[str, torch.Tensor]) -> Dict[str, Any]:
@@ -181,3 +191,79 @@ class MaskedLMModel(CaptioningModel):
             predictions[labels == self.padding_idx] = self.padding_idx
             output["predictions"] = predictions
         return output
+
+
+class ClassificationModel(_EngineModel):
+    """Drop-in for virtex/models/classification.py:12-108 on the same engine: a `LinearTextualHead` (global average pool
+    + one linear layer) over the backbone and the K-hot cross entropy
+
+        loss = mean_b( -mean_{u in U_b} log_softmax(logits_b)[u] ),   U_b = unique ids of batch["labels"][b] minus
+                                                                              ignore_indices,
+
+    NaN for a row whose U_b is empty (that row contributes no gradient).  In eval mode `predictions` holds the top-10
+    class ids of each image, int64 (B, 10).  Labels outside [0, vocab_size) are skipped; the reference would raise."""
+
+    def __init__(self, visual: VisualBackbone, textual: TextualHead, ignore_indices: List[int]):
+        super().__init__()
+        if not isinstance(textual, LinearTextualHead):
+            raise ValueError("the classification models run on a LinearTextualHead (MODEL.TEXTUAL.NAME 'none')")
+        self.visual = visual
+        self.textual = textual
+        self.ignore_indices = ignore_indices
+        self._engine = None
+
+    def _new_engine(self) -> Engine:
+        return Engine(self.visual, self.textual, ignore_indices=self.ignore_indices)
+
+    def forward(self, batch: Dict[str, torch.Tensor]) -> Dict[str, Any]:
+        image = batch["image"]
+        if image.device.type != "cuda":
+            raise RuntimeError("virtex_b200 has no CPU path: the batch must live on the model's CUDA device")
+        image = image.contiguous().float()
+        labels = batch["labels"]
+        labels = (labels if labels.dtype == torch.int64 else labels.long()).contiguous()
+        eng = self.engine
+        eng.mark_weights_dirty()
+        if self.training and torch.is_grad_enabled():
+            loss, _ = _StepFunction.apply(self, image, None, None, None, labels, *self._engine_params)
+        else:
+            loss = eng.forward(image, None, None, None, training=self.training, with_grad=False,
+                               labels=labels).clone()[0]
+        output: Dict[str, Any] = {"loss": loss, "loss_components": {"classification": loss.detach().clone()}}
+        if not self.training:
+            output["predictions"] = eng.predictions().clone()
+        return output
+
+    def _eval_predictions(self, batch):
+        self.eval()
+        with torch.no_grad():
+            predictions = self.forward(batch)["predictions"]
+        self.train()
+        return predictions
+
+
+class TokenClassificationModel(ClassificationModel):
+    """Targets: the unique caption tokens of each image, special tokens ignored."""
+
+    def log_predictions(self, batch: Dict[str, torch.Tensor], tokenizer) -> str:
+        """Caption and top-10 predicted tokens per image; `tokenizer` needs only `decode` and `id_to_token`."""
+        text = ""
+        for tokens, preds in zip(batch["caption_tokens"], self._eval_predictions(batch)):
+            names = " ".join(tokenizer.id_to_token(p) for p in preds.tolist())
+            text += (f"\n                Caption tokens : {tokenizer.decode(tokens.tolist())}"
+                     f"\n                Predictions (f): {names}\n\n                ")
+        return text
+
+
+class MultiLabelClassificationModel(ClassificationModel):
+    """Targets: the unique instance categories of each image, background (id 0) ignored."""
+
+    def log_predictions(self, batch: Dict[str, torch.Tensor], tokenizer=None) -> str:
+        """Sorted ground-truth category ids (background dropped) beside as many sorted top predictions."""
+        text = ""
+        for tokens, preds in zip(batch["caption_tokens"], self._eval_predictions(batch)):
+            gt = sorted(t for t in tokens.tolist() if t != 0)
+            pred = sorted(preds.tolist()[:len(gt)])
+            text += (f"\n                COCO Instance IDs (GT)   : {gt}"
+                     f"\n                COCO Instance IDs (Pred) : {pred}\n\n                ")
+        return text

@@ -162,6 +162,21 @@ class TextualHead(nn.Module):
         return self.hidden_size
 
 
+class LinearTextualHead(TextualHead):
+    """Drop-in for virtex/modules/textual_heads.py:46-95: global average pooling of the visual features, then one
+    `nn.Linear(visual_feature_size, vocab_size)` (default init).  The head of the classification pretext models."""
+
+    def __init__(self, visual_feature_size: int, vocab_size: int, **kwargs):
+        super().__init__(visual_feature_size, vocab_size, visual_feature_size)  # hidden_size = visual_feature_size
+        self.output = nn.Linear(visual_feature_size, vocab_size)
+
+    def forward(self, visual_features: torch.Tensor, caption_tokens: Optional[torch.Tensor] = None,
+                caption_lengths: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """(B, C, h, w) -> fp32 logits (B, V); the caption arguments are accepted and ignored, like the reference's."""
+        from .engine import linear_head_logits
+        return linear_head_logits(self, visual_features)
+
+
 class TransformerDecoderTextualHead(TextualHead):
     """Drop-in for virtex/modules/textual_heads.py:98-292 (same kwargs, attributes and initialisation)."""
 

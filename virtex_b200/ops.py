@@ -50,6 +50,10 @@ _PROTOS = {
     "vtx_cross_entropy": [P, I64, P, I, I, I, I, I, P, P, I, P],
     "vtx_colsum": [P, I64, I, I, P, P],
     "vtx_argmax_rows": [P, I64, I, I, P, P],
+    "vtx_group_mean_fwd": [P, P, I, I, I, P],
+    "vtx_group_mean_bwd": [P, P, I, I, I, P],
+    "vtx_khot_xent": [P, I64, P, I64, I, I, I, P, I, P, I, P],
+    "vtx_topk_rows": [P, I64, I, I, I, P, P],
     "vtx_image_resample": [P, P, P, P, P, P, I, I, P],
     "vtx_image_gray_sum": [P, P, P, P, I, I, P],
     "vtx_image_jitter_normalize": [P, P, P, P, P, P, I, I, P],

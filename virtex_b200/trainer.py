@@ -132,9 +132,12 @@ class Trainer:
                                "create a new Trainer, this one would update a stale parameter arena")
         eng.seed.add_(1)
         m = self.model
-        loss = eng.forward(batch["image"], batch["caption_tokens"],
-                           batch["noitpac_tokens"] if m.caption_backward else batch["caption_tokens"],
-                           batch["caption_lengths"], training=True, with_grad=True)
+        if eng.classify:  # token / multilabel classification: loss slots [loss, 0]
+            loss = eng.forward(batch["image"], None, None, None, training=True, with_grad=True, labels=batch["labels"])
+        else:
+            loss = eng.forward(batch["image"], batch["caption_tokens"],
+                               batch["noitpac_tokens"] if m.caption_backward else batch["caption_tokens"],
+                               batch["caption_lengths"], training=True, with_grad=True)
         eng.backward(zero_grads=True, bucket_cb=self._on_bucket if self.world > 1 else None)
         for w in self._pending:
             w.wait()
