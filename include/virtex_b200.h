@@ -103,6 +103,15 @@ typedef struct VtxGemm {
   float* bnr_sums;
   const uint8_t* bnr_mask;
   int64_t bnr_ldy;
+  /* Eval-mode BatchNorm folded into the epilogue (col_scale and col_shift both non-NULL, fp32 [N], 8-byte aligned): the
+         D[m, n] = bf16( act( fmaf(acc, col_scale[n], col_shift[n]) + residual[m, n] ) )
+     of a torchvision Bottleneck conv + BN (+ shortcut) (+ ReLU) in eval mode (torchvision resnet.py:146-163), with
+     scale / shift = rows 2 / 3 of the bnp vtx_bn_finalize writes with training = 0.  Needs a bf16 output, alpha 1,
+     act 0 or 1, N % 2 == 0, conv_mode 0 or 1 without an output view, no bias / stats / bnr_* / residual_mask, and a
+     residual (optional) that is 16-byte aligned with ldr % 8 == 0; anything else is rejected.  Both NULL: the epilogue
+     order above. */
+  const float* col_scale;
+  const float* col_shift;
 } VtxGemm;
 
 int vtx_gemm(const VtxGemm* g, void* stream);

@@ -119,6 +119,9 @@ struct GemmKParams {
   int bnr_prefetch;          // pull the y tile into L2 with a TMA prefetch when the tile starts
   int bnr;                   // 0: plain statistics (or none), 1: BN-backward sums, ReLU mask from y, 2: from a bit mask
   int trans_d;               // fp32 output stored transposed: D[col * ldd + row] (conv_mode 4)
+  // folded eval-mode BatchNorm (kernel variant SS): per-column affine map of the accumulators, [N] each
+  const float* col_scale;
+  const float* col_shift;
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
@@ -248,7 +251,10 @@ __device__ __forceinline__ void mma_tile(float* acc, uint8_t* smem, const GemmKP
 //         accumulators per thread), taking every other slot of the tile-index ring.  A pair of barriers makes the two
 //         K loops alternate whole tiles, so one warpgroup's epilogue runs while the other one's MMAs do.  Each
 //         warpgroup has its own staging buffer, residual barrier, named barrier and BN-statistics partials.
-template <int BN, bool PP>
+// SS selects the epilogue: false runs the loops below for every option; true runs only the scale / shift loop of a
+// folded eval-mode BatchNorm (p.col_scale / p.col_shift, optional TMA-staged residual, optional ReLU).  A variant of
+// its own keeps that loop out of the training instantiations, whose register allocation it would otherwise perturb.
+template <int BN, bool PP, bool SS>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmR,
@@ -588,7 +594,40 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int r_ = mt * kBM + r;
       return r_ < p.M ? (long long)r_ : -1;
     };
-    if (bias_only) {
+    if constexpr (SS) {
+      // folded eval-mode BatchNorm: bf16_rn(act(fmaf(acc, scale, shift) + residual)), laid out like the bias loop:
+      // one float2 of scale and one of shift and one swizzled address per column pair j serve every row the thread
+      // holds; pairs at or past N (N is even) read zeros and are clipped by the TMA store.  The residual is the tile
+      // the TMA staged in this buffer (rows outside the output are zero filled).
+      const uint32_t srow = smem_u32(cbuf) + ((PP ? 0 : wg) * 64 + wl * 16 + (lane >> 2)) * 128 + q * 4;
+      const int sw = lane >> 2;
+      const int col0 = n_base + 2 * q;
+      const bool res = p.res_tma != 0, relu = p.act == 1;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = col0 + 8 * j;
+        const bool in = col < p.N;
+        const float2 sc = in ? __ldg(reinterpret_cast<const float2*>(p.col_scale + col)) : make_float2(0.f, 0.f);
+        const float2 sh = in ? __ldg(reinterpret_cast<const float2*>(p.col_shift + col)) : make_float2(0.f, 0.f);
+        const uint32_t sa = srow + (j >> 3) * 16384 + (((j & 7) ^ sw) << 4);
+#pragma unroll
+        for (int hh = 0; hh < 2 * NH; ++hh) {
+          const float* accb = acc + (hh >> 1) * (BN / 2) + 4 * j + 2 * (hh & 1);
+          const uint32_t a = sa + ((hh >> 1) * 64 + 8 * (hh & 1)) * 128;
+          float v0 = fmaf(accb[0], sc.x, sh.x), v1 = fmaf(accb[1], sc.y, sh.y);
+          if (res) {
+            const uint32_t r = lds32(a);  // bf16 pair: low half is column col, high half col + 1
+            v0 += __uint_as_float(r << 16);
+            v1 += __uint_as_float(r & 0xffff0000u);
+          }
+          if (relu) {
+            v0 = fmaxf(v0, 0.f);
+            v1 = fmaxf(v1, 0.f);
+          }
+          sts32(a, pack_bf16x2(v0, v1));
+        }
+      }
+    } else if (bias_only) {
       // bf16 output + bias: fp32(acc + bias) rounded once to bf16, as the general loop computes it (alpha == 1 makes
       // its multiplication exact, fused or not).  A thread's columns 8 j + 2 q are the same in every row it holds, so
       // one bias pair per j serves all of them; pairs at or past N (N is even) read zeros and are clipped by the TMA
@@ -976,6 +1015,19 @@ static void choose_box(int H, int W, int positions, int* bw, int* bh, int* bn) {
   *bw = best_w; *bh = best_h; *bn = positions / (best_w * best_h);
 }
 
+// the instantiation of a launch: tile width, schedule and epilogue variant
+template <bool SS>
+static cudaError_t launch_gemm(const cudaLaunchConfig_t& cfg, bool pingpong, int bn, const CUtensorMap& tmA,
+                               const CUtensorMap& tmB, const CUtensorMap& tmD, const CUtensorMap& tmR,
+                               const CUtensorMap& tmY, const GemmKParams& p) {
+  if (pingpong && bn == 64) return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64, true, SS>, tmA, tmB, tmD, tmR, tmY, p);
+  if (pingpong) return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128, true, SS>, tmA, tmB, tmD, tmR, tmY, p);
+  if (bn == 64) return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64, false, SS>, tmA, tmB, tmD, tmR, tmY, p);
+  if (bn == 128) return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128, false, SS>, tmA, tmB, tmD, tmR, tmY, p);
+  if (bn == 192) return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<192, false, SS>, tmA, tmB, tmD, tmR, tmY, p);
+  return cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<256, false, SS>, tmA, tmB, tmD, tmR, tmY, p);
+}
+
 }  // namespace vtx
 
 using namespace vtx;
@@ -1115,6 +1167,20 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     p.bnr_prefetch = (pf != nullptr && pf[0] == '0') ? 0 : 1;
     p.bnr = g->bnr_mask == nullptr ? 1 : 2;
   }
+  // folded eval-mode BatchNorm: the scale / shift variant, whose only epilogue is act(acc * scale + shift + residual)
+  const bool ss = g->col_scale != nullptr || g->col_shift != nullptr;
+  if (ss) {
+    if (!g->col_scale || !g->col_shift || g->out_f32 || (g->alpha != 0.f && g->alpha != 1.f) || g->bias || g->stats ||
+        bnr || g->act < 0 || g->act > 1 || g->N % 2 != 0 || (reinterpret_cast<uintptr_t>(g->col_scale) & 7) != 0 ||
+        (reinterpret_cast<uintptr_t>(g->col_shift) & 7) != 0 || g->residual_mask || g->conv_out_w > 0 ||
+        (g->conv_mode != 0 && g->conv_mode != 1) ||
+        (g->residual && (g->ldr % 8 != 0 || (reinterpret_cast<uintptr_t>(g->residual) & 15) != 0)))
+      return set_error(VTX_EINVAL, "vtx_gemm: col_scale / col_shift need both vectors 8-byte aligned, a bf16 output, "
+                                   "alpha 1, act 0 or 1, N %% 2 == 0, conv_mode 0 or 1 without an output view, no bias / "
+                                   "stats / bnr / residual mask, and a 16-byte aligned residual with ldr %% 8 == 0");
+    p.col_scale = g->col_scale;
+    p.col_shift = g->col_shift;
+  }
 
   CUtensorMap tmA, tmB;
   int rc;
@@ -1218,10 +1284,11 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   memset(&tmD, 0, sizeof(tmD));
   memset(&tmR, 0, sizeof(tmR));
   // the TMA-staged residual is added in packed bf16 AFTER the accumulator is rounded, which is only the documented
-  // order (alpha * acc + bias + residual, then the activation) when there is nothing else in the epilogue
+  // order (alpha * acc + bias + residual, then the activation) when there is nothing else in the epilogue; the scale /
+  // shift variant adds it in fp32 before its ReLU
   p.res_tma = (p.cbytes && g->residual != nullptr && g->ldr % 8 == 0 &&
                (reinterpret_cast<uintptr_t>(g->residual) & 15) == 0 && p.alpha == 1.0f && g->bias == nullptr &&
-               g->act == 0) ? 1 : 0;
+               (g->act == 0 || ss)) ? 1 : 0;
   if (p.cbytes) {
     if (p.mode & 1) {
       uint64_t dd[4] = {(uint64_t)g->N, (uint64_t)p.cW, (uint64_t)p.cH, (uint64_t)g->conv_n};
@@ -1273,10 +1340,14 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !attr_set[dev]) {
       cudaError_t e = cudaSuccess;
-      const void* kernels[6] = {(const void*)gemm_wgmma_kernel<64, false>,  (const void*)gemm_wgmma_kernel<128, false>,
-                                (const void*)gemm_wgmma_kernel<192, false>, (const void*)gemm_wgmma_kernel<256, false>,
-                                (const void*)gemm_wgmma_kernel<64, true>,   (const void*)gemm_wgmma_kernel<128, true>};
-      for (int i = 0; i < 6 && e == cudaSuccess; ++i)
+      const void* kernels[12] = {
+          (const void*)gemm_wgmma_kernel<64, false, false>,  (const void*)gemm_wgmma_kernel<128, false, false>,
+          (const void*)gemm_wgmma_kernel<192, false, false>, (const void*)gemm_wgmma_kernel<256, false, false>,
+          (const void*)gemm_wgmma_kernel<64, true, false>,   (const void*)gemm_wgmma_kernel<128, true, false>,
+          (const void*)gemm_wgmma_kernel<64, false, true>,   (const void*)gemm_wgmma_kernel<128, false, true>,
+          (const void*)gemm_wgmma_kernel<192, false, true>,  (const void*)gemm_wgmma_kernel<256, false, true>,
+          (const void*)gemm_wgmma_kernel<64, true, true>,    (const void*)gemm_wgmma_kernel<128, true, true>};
+      for (int i = 0; i < 12 && e == cudaSuccess; ++i)
         e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal);
       if (e != cudaSuccess) return set_error(VTX_ECUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
       if (dev >= 0 && dev < 64) attr_set[dev] = true;
@@ -1311,13 +1382,8 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cudaError_t le;
-    if (pingpong && bn == 64) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64, true>, tmA, tmB, tmD, tmR, tmY, p);
-    else if (pingpong) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128, true>, tmA, tmB, tmD, tmR, tmY, p);
-    else if (bn == 64) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<64, false>, tmA, tmB, tmD, tmR, tmY, p);
-    else if (bn == 128) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<128, false>, tmA, tmB, tmD, tmR, tmY, p);
-    else if (bn == 192) le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<192, false>, tmA, tmB, tmD, tmR, tmY, p);
-    else le = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<256, false>, tmA, tmB, tmD, tmR, tmY, p);
+    const cudaError_t le = ss ? launch_gemm<true>(cfg, pingpong, bn, tmA, tmB, tmD, tmR, tmY, p)
+                              : launch_gemm<false>(cfg, pingpong, bn, tmA, tmB, tmD, tmR, tmY, p);
     if (le != cudaSuccess) return set_error(VTX_ECUDA, "gemm_wgmma_kernel PDL launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();

@@ -160,6 +160,7 @@ class Engine:
         self._tape = None
         self.generation = 0  # bumped by every forward(): a backward must match the forward that filled the tape
         self._weights_fresh = False
+        self._eval_bn_fresh = False  # the running-statistics scale / shift of every BN (backbone_infer's epilogues)
         # BN-backward reductions (sum dz, sum dz * xhat) accumulated by the epilogue of the GEMM that produces the
         # gradient (bn1 / bn2 of every block, bn3 of blocks followed by an identity block) instead of a separate pass;
         # VTX_BNR_FUSE=0 is the measurement knob for the A/B against the standalone vtx_bn_bwd_reduce launches
@@ -179,6 +180,7 @@ class Engine:
 
     def mark_weights_dirty(self):
         self._weights_fresh = False
+        self._eval_bn_fresh = False
 
     def _build_backbone_plan(self):
         self.blocks = []
@@ -265,13 +267,28 @@ class Engine:
                 rows.append((self._dwp["visual.cnn.conv1"], g, 64 * 147, 64, 3, 7, 7, 160, 2))
         return rows
 
-    def prepare_weights(self, mirror=True):
-        """bf16 mirror of all parameters + packed GEMM layouts of the k>1 convolution weights."""
+    def prepare_weights(self, mirror=True, eval_bn=False):
+        """bf16 mirror of all parameters + packed GEMM layouts of the k>1 convolution weights.  `eval_bn`: also the
+        eval-mode bnp [4, C] = mean, invstd, scale, shift of every BN from its running statistics (backbone_infer)."""
         if mirror:
             self.arena.refresh_mirror()
         if self.visual is not None:
             self._run_jobs("pack", self._pack_rows)  # every packed conv-weight layout in one launch
+            if eval_bn:
+                for bn_name, C in self._bn_names():
+                    self._bn_fwd(None, bn_name, 1, C, False, None, key="bnp_eval:")
+                self._eval_bn_fresh = True
         self._weights_fresh = True
+
+    def _bn_names(self):
+        """(name, channels) of every BatchNorm of the backbone."""
+        out = [("visual.cnn.bn1", 64)]
+        for name, blk in self.blocks:
+            planes = blk.conv1.weight.shape[0]
+            out += [(name + ".bn1", planes), (name + ".bn2", planes), (name + ".bn3", 4 * planes)]
+            if blk.downsample is not None:
+                out.append((name + ".downsample.1", 4 * planes))
+        return out
 
     def _pack_buf(self, key, shape):
         t = self._packed.get(key)
@@ -281,8 +298,8 @@ class Engine:
         return t
 
     # ------------------------------------------------------------------------------------------------ backbone fwd
-    def _bn_fwd(self, y, bn_name, M, C, training, stats):
-        bnp = self.ws.get("bnp:" + bn_name, (4, C), F32)
+    def _bn_fwd(self, y, bn_name, M, C, training, stats, key="bnp:"):
+        bnp = self.ws.get(key + bn_name, (4, C), F32)
         nbt = self.buffers[bn_name + ".num_batches_tracked"]
         call("vtx_bn_finalize", _p(stats), float(M), self.P(bn_name + ".weight").data_ptr(),
              self.P(bn_name + ".bias").data_ptr(), self.buffers[bn_name + ".running_mean"].data_ptr(),
@@ -321,6 +338,8 @@ class Engine:
         """image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, 2048]; fills the tape used by backward."""
         if not self._weights_fresh:
             self.prepare_weights()
+        if training:
+            self._eval_bn_fresh = False  # the running statistics move
         B, _, H, W = image.shape
         s = _stream()
         ws = self.ws
@@ -415,6 +434,80 @@ class Engine:
         tape["hw"] = (Hc, Wc)
         tape["C"] = Cin
         self._tape = tape
+        return x, Hc, Wc
+
+    def backbone_infer(self, image: torch.Tensor):
+        """Eval-mode backbone forward: image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, 2048].
+        Every BN is the fixed per-channel affine map of its running statistics, applied by the epilogue of the GEMM
+        that produces its input (VtxGemm.col_scale / col_shift), together with the shortcut and the ReLU: no raw conv
+        output is stored and read back.  Writes no tape and no statistics; its buffers are its own, so a training
+        tape stays intact.  The result is overwritten by the next call."""
+        if not self._weights_fresh or not self._eval_bn_fresh:
+            self.prepare_weights(eval_bn=True)
+        B, _, H, W = image.shape
+        s = _stream()
+        ws = self.ws
+
+        def ss(bn_name):  # scale and shift rows of the eval bnp
+            bnp = ws.flat["bnp_eval:" + bn_name]
+            C = bnp.numel() // 4
+            return dict(col_scale=bnp[2 * C:3 * C], col_shift=bnp[3 * C:4 * C])
+
+        # ---- stem: GEMM -> BN + ReLU + maxpool, as in backbone_forward
+        Ho, Wo = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
+        M0 = B * Ho * Wo
+        y0 = ws.get("inf.stem.y", (M0, 64), BF16)
+        if H % 2 == 0 and W % 4 == 0 and Ho % 8 == 0 and Wo % 16 == 0:
+            s2d = ws.get("inf.stem.s2d", (B, H // 2 + 3, W // 2 + 3, 16), BF16)
+            call("vtx_stem_s2d", image.data_ptr(), s2d.data_ptr(), B, H, W, s)
+            gemm(s2d, self._packed["visual.cnn.conv1.weight#s2d"], y0, M0, 64, 256, lda=64, ldb=256,
+                 conv=(B, Ho, Wo, 64), conv_mode=5)
+        else:
+            cols = ws.get("inf.stem.cols", (M0, 160), BF16)
+            call("vtx_stem_im2col", image.data_ptr(), cols.data_ptr(), B, H, W, 160, s)
+            gemm(cols, self._packed["visual.cnn.conv1.weight"], y0, M0, 64, 160)
+        Hp, Wp = (Ho - 1) // 2 + 1, (Wo - 1) // 2 + 1
+        x = ws.get("inf.x1", (B * Hp * Wp, 64), BF16)
+        idx = ws.get("inf.stem.idx", (B * Hp * Wp, 64), torch.uint8)
+        call("vtx_bn_relu_maxpool", y0.data_ptr(), ws.flat["bnp_eval:visual.cnn.bn1"].data_ptr(), x.data_ptr(),
+             idx.data_ptr(), B, Ho, Wo, 64, s)
+        Hc, Wc, Cin = Hp, Wp, 64
+        # ---- bottleneck blocks: four GEMMs, each ending in its BN (+ shortcut) (+ ReLU); block outputs alternate
+        # between two buffers
+        for bi, (name, blk) in enumerate(self.blocks):
+            planes = blk.conv1.weight.shape[0]
+            stride = blk.stride
+            Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
+            Min, Mout, C4 = B * Hc * Wc, B * Hn * Wn, 4 * planes
+            a1 = ws.get("inf.a1", (Min, planes), BF16)
+            gemm(x, self.W(name + ".conv1.weight").view(planes, Cin), a1, Min, planes, Cin, act=1, **ss(name + ".bn1"))
+            a2 = ws.get("inf.a2", (Mout, planes), BF16)
+            w2 = self._packed[name + ".conv2.weight"]
+            if planes % 64 == 0:
+                gemm(a1, w2, a2, Mout, planes, 9 * planes, lda=planes, conv=(B, Hc, Wc, planes), conv_mode=1,
+                     conv_stride=stride, act=1, **ss(name + ".bn2"))
+            else:
+                cols2 = ws.get("inf.cols2", (Mout, 9 * planes), BF16)
+                call("vtx_im2col3x3", a1.data_ptr(), cols2.data_ptr(), B, Hc, Wc, planes, stride, s)
+                gemm(cols2, w2, a2, Mout, planes, 9 * planes, act=1, **ss(name + ".bn2"))
+            shortcut = x
+            if blk.downsample is not None:
+                shortcut = ws.get("inf.shortcut", (Mout, C4), BF16)
+                wd = self.W(name + ".downsample.0.weight").view(C4, Cin)
+                sd = ss(name + ".downsample.1")
+                if stride == 1:
+                    gemm(x, wd, shortcut, Mout, C4, Cin, **sd)
+                elif Cin % 64 == 0:
+                    gemm(x, wd, shortcut, Mout, C4, Cin, lda=Cin, conv=(B, Hc, Wc, Cin), conv_mode=1, conv_stride=stride,
+                         conv_taps=1, **sd)
+                else:
+                    xs = ws.get("inf.xs", (Mout, Cin), BF16)
+                    call("vtx_subsample", x.data_ptr(), xs.data_ptr(), B, Hc, Wc, Cin, stride, s)
+                    gemm(xs, wd, shortcut, Mout, C4, Cin, **sd)
+            out = ws.get(f"inf.x{bi & 1}", (Mout, C4), BF16)
+            gemm(a2, self.W(name + ".conv3.weight").view(C4, planes), out, Mout, C4, planes, residual=shortcut, act=1,
+                 **ss(name + ".bn3"))
+            x, Hc, Wc, Cin = out, Hn, Wn, C4
         return x, Hc, Wc
 
     # ------------------------------------------------------------------------------------------------ backbone bwd
@@ -850,6 +943,10 @@ class Engine:
         W, dW, db = self.W(wname), self.G(wname), self.G(bname)
         if w_rows is not None:
             W, dW, db = W[w_rows], dW[w_rows], db[w_rows]
+        self._linear_bwd_t(dY, X, W, dW, db, dX, M, n_out, k_in, residual)
+
+    def _linear_bwd_t(self, dY, X, W, dW, db, dX, M, n_out, k_in, residual=None):
+        """The same for explicit tensors: bf16 W [n_out, k_in]; fp32 dW, db accumulated into."""
         call("vtx_colsum", dY.data_ptr(), dY.stride(0), M, n_out, db.data_ptr(), _stream())
         self._wgrad(dY, X, dW, n_out, k_in, M)
         if dX is not None:
@@ -1087,6 +1184,144 @@ def backbone_features(backbone, image: torch.Tensor) -> torch.Tensor:
     out = torch.empty(B, C, h, w, dtype=F32, device=image.device)
     call("vtx_nhwc_to_nchw_f32", feat.data_ptr(), out.data_ptr(), B, h * w, C, _stream())
     return out
+
+
+class _CnnView:
+    """A stand-alone ResNetParams as an engine's `visual`: its backbone parameters under the names the engine uses
+    ('visual.cnn.*'), without `fc`, which its forward may replace at any time and reads afresh on every call."""
+
+    frozen = False
+
+    def __init__(self, cnn):
+        self.cnn = cnn
+
+    def named_parameters(self):
+        return [("cnn." + n, p) for n, p in self.cnn.named_parameters() if not n.startswith("fc.")]
+
+    def named_buffers(self):
+        return [("cnn." + n, b) for n, b in self.cnn.named_buffers() if not n.startswith("fc.")]
+
+
+def _cnn_engine(cnn):
+    eng = cnn.__dict__.get("_vtx_engine")
+    if eng is None or not eng.arena.intact():
+        eng = Engine(visual=_CnnView(cnn))
+        object.__setattr__(cnn, "_vtx_engine", eng)
+    return eng
+
+
+def _fc_of(cnn):
+    fc = cnn.fc
+    if isinstance(fc, nn.Identity):
+        return None
+    if not isinstance(fc, nn.Linear) or fc.bias is None:
+        raise TypeError(f"ResNetParams.fc must be nn.Identity or nn.Linear with a bias, not {type(fc).__name__}")
+    if fc.weight.device != cnn.conv1.weight.device:
+        raise RuntimeError("ResNetParams.fc is not on the backbone's device: move it with .to(device)")
+    return fc
+
+
+def _resnet_pool_fc(eng, feat, B, hw, fc_w, fc_b):
+    """Global average pool of the NHWC features (vtx_group_mean_fwd) and the fc GEMM -> (fp32 output, bf16 pooled,
+    bf16 fc weight).  fc_w None: the output is the pooled features."""
+    C = feat.shape[1]
+    pooled = eng.ws.get("fc.pooled", (B, C), BF16)
+    call("vtx_group_mean_fwd", feat.data_ptr(), pooled.data_ptr(), B, hw, C, _stream())
+    if fc_w is None:
+        return pooled.float(), pooled, None
+    N = fc_w.shape[0]
+    w = eng.ws.get("fc.weight_bf16", (N, C), BF16)  # cast on every call: the optimiser updates fc in place
+    call("vtx_cast_bf16", fc_w.data_ptr(), w.data_ptr(), N * C, _stream())
+    out = torch.empty(B, _round_up(N, 4), dtype=F32, device=feat.device)  # fp32 rows stay 16-byte aligned
+    gemm(pooled, w, out, B, N, C, bias=fc_b)
+    return out[:, :N], pooled, w
+
+
+def _resnet_run(cnn, image, fc_w, fc_b):
+    """Backbone (train mode: the training backbone_forward with batch statistics and the running-statistics update;
+    eval mode: backbone_infer), pool and fc -> (fp32 output, engine, bf16 pooled, bf16 fc weight, h * w)."""
+    eng = _cnn_engine(cnn)
+    if cnn.training:
+        eng.mark_weights_dirty()  # parameters may have been updated by any optimiser since the last call
+        feat, h, w = eng.backbone_forward(image, training=True)
+        eng.mark_weights_dirty()  # the running statistics moved
+    else:
+        feat, h, w = eng.backbone_infer(image)
+    out, pooled, wb = _resnet_pool_fc(eng, feat, image.shape[0], h * w, fc_w, fc_b)
+    return out, eng, pooled, wb, h * w
+
+
+class _ResNetFunction(torch.autograd.Function):
+    """ResNetParams.forward as one autograd node: gradients for fc (pool + linear backward) and, in train mode, for
+    the backbone parameters passed in `params` (backbone_backward)."""
+
+    @staticmethod
+    def forward(ctx, cnn, image, fc_w, fc_b, *params):
+        out, eng, pooled, wb, hw = _resnet_run(cnn, image, fc_w, fc_b)
+        eng.generation += 1
+        ctx.eng, ctx.generation, ctx.hw, ctx.n_params = eng, eng.generation, hw, len(params)
+        ctx.pooled, ctx.wb, ctx.has_fc = pooled.clone(), wb, fc_w is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        eng = ctx.eng
+        B, C = ctx.pooled.shape
+        s = _stream()
+        need_bb = ctx.n_params > 0
+        if need_bb and eng.generation != ctx.generation:
+            raise RuntimeError("the backbone ran another forward since this output was computed: its activation tape "
+                               "was overwritten; call backward() before the next forward")
+        dfc_w = dfc_b = None
+        dpooled = eng.ws.get("fc.dpooled", (B, C), BF16) if need_bb else None
+        if ctx.has_fc:
+            N = ctx.wb.shape[0]
+            ld = _round_up(N, 8)  # bf16 rows of the dlogits stay 16-byte aligned; the GEMMs' TMA zero-fills the K tail
+            g32 = eng.ws.get("fc.dlogits_f32", (B, ld), F32)
+            if ld != N:
+                g32.zero_()
+            g32[:, :N].copy_(g)
+            dY = eng.ws.get("fc.dlogits", (B, ld), BF16)
+            call("vtx_cast_bf16", g32.data_ptr(), dY.data_ptr(), B * ld, s)
+            dfc_w = torch.zeros(N, C, dtype=F32, device=g.device)
+            dfc_b = torch.zeros(N, dtype=F32, device=g.device)
+            eng._linear_bwd_t(dY, ctx.pooled, ctx.wb, dfc_w, dfc_b, dpooled, B, N, C)
+        elif need_bb:
+            call("vtx_cast_bf16", g.contiguous().data_ptr(), dpooled.data_ptr(), B * C, s)
+        grads = [None] * ctx.n_params
+        if need_bb:
+            dfeat = eng.ws.get("fc.dfeat", (B * ctx.hw, C), BF16)
+            call("vtx_group_mean_bwd", dpooled.data_ptr(), dfeat.data_ptr(), B, ctx.hw, C, s)
+            eng.arena.grads.zero_()
+            eng.backbone_backward(dfeat)
+            flat = eng.arena.grads.clone()  # the arena is reused by the next backward
+            grads = [eng.arena.view(flat, n) if need else None
+                     for n, need in zip(eng.arena.names, ctx.needs_input_grad[4:])]
+        return (None, None, dfc_w, dfc_b, *grads)
+
+
+def resnet_forward(cnn, image: torch.Tensor) -> torch.Tensor:
+    """`ResNetParams.forward`, as torchvision's ResNet.forward: image fp32 NCHW (B,3,H,W) -> fc(flatten(avgpool(layer4)))
+    in fp32, (B, num_classes) for an nn.Linear fc and the (B, 2048) pooled features for nn.Identity."""
+    _require_cuda(image.device)
+    image = image.contiguous().float()
+    fc = _fc_of(cnn)
+    fc_w = fc_b = None
+    if fc is not None:
+        fc_w, fc_b = fc.weight, fc.bias
+        if fc_w.dtype != F32 or fc_b.dtype != F32 or not fc_w.is_contiguous():
+            raise TypeError("ResNetParams.fc needs contiguous fp32 parameters")
+    eng = _cnn_engine(cnn)
+    params = [eng.arena._param_objs[n] for n in eng.arena.names]
+    grad = torch.is_grad_enabled()
+    if not cnn.training and grad and any(p.requires_grad for p in params):
+        raise RuntimeError("backward through eval-mode BatchNorm is not implemented: freeze the backbone "
+                           "(requires_grad = False) for an eval-mode forward with gradients, or run it under no_grad")
+    bb = params if cnn.training and any(p.requires_grad for p in params) else []
+    if grad and (bb or (fc is not None and (fc_w.requires_grad or fc_b.requires_grad))):
+        return _ResNetFunction.apply(cnn, image, fc_w, fc_b, *bb)
+    with torch.no_grad():
+        return _resnet_run(cnn, image, fc_w, fc_b)[0].clone()
 
 
 @torch.no_grad()

@@ -36,6 +36,7 @@ class VtxGemm(ctypes.Structure):
         ("ldd_w", c_i64), ("ldd_h", c_i64), ("ldd_n", c_i64),
         ("residual_mask", c_void_p),
         ("bnr_y", c_void_p), ("bnr_bnp", c_void_p), ("bnr_sums", c_void_p), ("bnr_mask", c_void_p), ("bnr_ldy", c_i64),
+        ("col_scale", c_void_p), ("col_shift", c_void_p),
     ]
 
 

@@ -41,7 +41,14 @@ class Bottleneck(_NoForward):
 
 
 class ResNetParams(_NoForward):
-    """Parameter tree of torchvision ResNet-50/101/152 up to layer4 (`fc` replaced by Identity as in the reference)."""
+    """Parameter tree of torchvision ResNet-50/101/152 up to layer4 (`fc` replaced by Identity as in the reference).
+
+    Callable like torchvision's ResNet (the downstream evaluations, scripts/clf_linear.py and scripts/clf_voc07.py):
+    `forward(image fp32 (B,3,H,W)) -> fc(flatten(avgpool(layer4)))` in fp32, the (B, 2048) pooled features while `fc`
+    is nn.Identity, logits once an nn.Linear is assigned to `fc`.  In eval mode every BatchNorm uses its running
+    statistics, folded into the GEMM epilogues (Engine.backbone_infer), and gradients reach `fc` only; the backbone
+    must then be frozen (requires_grad False) or the call made under no_grad.  In train mode BN uses batch statistics
+    and updates its running statistics, and every parameter gets its gradient."""
 
     def __init__(self, name: str = "resnet50", zero_init_residual: bool = True):
         super().__init__()
@@ -58,6 +65,7 @@ class ResNetParams(_NoForward):
                 blocks.append(Bottleneck(inplanes, planes, stride, downsample=(stride != 1 or inplanes != planes * 4)))
                 inplanes = planes * 4
             setattr(self, f"layer{li}", nn.Sequential(*blocks))
+        self.avgpool = nn.AdaptiveAvgPool2d((1, 1))  # torchvision's attribute (no state); forward pools in CUDA
         self.fc = nn.Identity()
         # torchvision/models/resnet.py:208-223
         for m in self.modules():
@@ -70,6 +78,17 @@ class ResNetParams(_NoForward):
             for m in self.modules():
                 if isinstance(m, Bottleneck):
                     nn.init.constant_(m.bn3.weight, 0)
+
+    def forward(self, image: torch.Tensor) -> torch.Tensor:
+        from .engine import resnet_forward
+        return resnet_forward(self, image)
+
+    def _load_from_state_dict(self, *args, **kwargs):
+        # new weights or running statistics: the engine re-derives its bf16 weights and folded BN parameters
+        super()._load_from_state_dict(*args, **kwargs)
+        eng = self.__dict__.get("_vtx_engine")
+        if eng is not None:
+            eng.mark_weights_dirty()
 
 
 class VisualBackbone(nn.Module):

@@ -133,13 +133,16 @@ _gemm_struct = L.VtxGemm()
 
 def gemm(A, B, D, M, N, K, *, lda=None, ldb=None, ldd=None, a_mn=0, b_mn=0, bias=None, act=0, residual=None,
          ldr=0, stats=None, atomic=False, split_k=1, tile_n=0, conv=None, conv_mode=0, out_f32=None, residual_mask=None,
-         conv_stride=1, conv_taps=0, tap_grid=None, out_view=None, d_ptr=None, bnr=None):
+         conv_stride=1, conv_taps=0, tap_grid=None, out_view=None, d_ptr=None, bnr=None, col_scale=None,
+         col_shift=None):
     """D[M,N] = epilogue(A . B^T) through the wgmma kernel; see include/virtex_b200.h (VtxGemm).
-    bnr = (y, bnp, sums, mask or None[, y_ptr]): BN-backward reduction of the output fused into the epilogue."""
+    bnr = (y, bnp, sums, mask or None[, y_ptr]): BN-backward reduction of the output fused into the epilogue.
+    col_scale / col_shift (fp32 [N]): eval-mode BatchNorm folded into the epilogue, act(acc * scale + shift + residual)."""
     g = _gemm_struct
     g.A, g.B, g.D = A.data_ptr(), B.data_ptr(), (D.data_ptr() if d_ptr is None else d_ptr)
     g.bias, g.residual, g.stats = _p(bias), _p(residual), _p(stats)
     g.residual_mask = _p(residual_mask)
+    g.col_scale, g.col_shift = _p(col_scale), _p(col_shift)
     g.lda = A.stride(0) if lda is None else lda
     g.ldb = B.stride(0) if ldb is None else ldb
     g.ldd = D.stride(0) if ldd is None else ldd
