@@ -316,8 +316,9 @@ def _gelu(x):
     return 0.5 * x * (1.0 + torch.erf(x * (1.0 / math.sqrt(2.0))))
 
 
-def _mha(P, prefix, x_q, x_kv, heads, bias_mask, self_attn):
-    """Packed in-projection multi-head attention; bias_mask broadcastable to (B, heads, Tq, Tk) or None."""
+def _mha(P, prefix, x_q, x_kv, heads, bias_mask, self_attn, drop=None, site=0):
+    """Packed in-projection multi-head attention; bias_mask broadcastable to (B, heads, Tq, Tk) or None.
+    `drop(probs, site)` (optional) is the dropout of the (B, heads, Tq, Tk) attention probabilities."""
     H = x_q.shape[-1]
     W, bvec = P[prefix + ".in_proj_weight"], P[prefix + ".in_proj_bias"]
     if self_attn:
@@ -337,12 +338,22 @@ def _mha(P, prefix, x_q, x_kv, heads, bias_mask, self_attn):
     if bias_mask is not None:
         s = s + bias_mask
     pr = torch.softmax(s, dim=-1)
+    if drop is not None:
+        pr = drop(pr, site)
     o = (pr @ v).transpose(1, 2).reshape(B, Tq, H)
     return o @ P[prefix + ".out_proj.weight"].t() + P[prefix + ".out_proj.bias"]
 
 
-def head_forward(P, visual_features, tokens, lengths, spec: Spec, direction: str = "textual"):
-    """(B,C,h,w), (B,T) int64, (B,) int64 -> logits (B,T,V).  Dropout is the identity (p = 0 / eval)."""
+def head_forward(P, visual_features, tokens, lengths, spec: Spec, direction: str = "textual", drop=None):
+    """(B,C,h,w), (B,T) int64, (B,) int64 -> logits (B,T,V).  Dropout is the identity (p = 0 / eval) unless `drop` is
+    given: `drop(x, site)` is then applied at the reference's 7 dropout points, numbered as the CUDA engine numbers its
+    dropout sites (di = 0 for "textual", 1 for "backward_textual"; sb = di * 1000 + 10 * (layer + 1)):
+      embedding output after its LayerNorm, before the pad mask     di * 1000    x (B, T, H)
+      self- / cross-attention probabilities                         sb + 0 / 2   x (B, heads, Tq, Tk)
+      dropout1 / 2 / 3 of the residual branches                     sb + 1 / 3 / 5  x (B, T, H)
+      the feed-forward hidden after GELU                            sb + 4       x (B, T, F)"""
+    drop_ = drop if drop is not None else (lambda x, site: x)
+    di = 0 if direction == "textual" else 1
     B, C, h, w = visual_features.shape
     vf = visual_features.reshape(B, C, h * w).permute(0, 2, 1)
     mem = vf @ P["textual.visual_projection.weight"].t() + P["textual.visual_projection.bias"]
@@ -350,6 +361,7 @@ def head_forward(P, visual_features, tokens, lengths, spec: Spec, direction: str
     # embedding (virtex/modules/embedding.py:58-73)
     emb = P["textual.embedding.words.weight"][tokens] + P["textual.embedding.positions.weight"][:T][None]
     emb = _layer_norm(emb, P["textual.embedding.layer_norm.weight"], P["textual.embedding.layer_norm.bias"], 1e-8)
+    emb = drop_(emb, di * 1000)
     emb = emb * (tokens != spec.pad).unsqueeze(-1).to(emb.dtype)
     # masks
     pos = torch.arange(1, T + 1)[None, :]
@@ -361,20 +373,22 @@ def head_forward(P, visual_features, tokens, lengths, spec: Spec, direction: str
     x = emb
     for l in range(spec.layers):
         q = f"{direction}.transformer.layers.{l}."
+        sb = di * 1000 + 10 * (l + 1)
         n1 = lambda t: _layer_norm(t, P[q + "norm1.weight"], P[q + "norm1.bias"], 1e-5)
         n2 = lambda t: _layer_norm(t, P[q + "norm2.weight"], P[q + "norm2.bias"], 1e-5)
         n3 = lambda t: _layer_norm(t, P[q + "norm3.weight"], P[q + "norm3.bias"], 1e-5)
-        ff = lambda t: _gelu(t @ P[q + "linear1.weight"].t() + P[q + "linear1.bias"]) @ P[q + "linear2.weight"].t() \
-            + P[q + "linear2.bias"]
+        ff = lambda t: drop_(_gelu(t @ P[q + "linear1.weight"].t() + P[q + "linear1.bias"]), sb + 4) \
+            @ P[q + "linear2.weight"].t() + P[q + "linear2.bias"]
+        sa = lambda t: drop_(_mha(P, q + "self_attn", t, t, spec.heads, bias, True, drop, sb + 0), sb + 1)
+        ca = lambda t: drop_(_mha(P, q + "multihead_attn", t, mem, spec.heads, None, False, drop, sb + 2), sb + 3)
         if spec.norm_first:
-            y = n1(x)
-            x = x + _mha(P, q + "self_attn", y, y, spec.heads, bias, True)
-            x = x + _mha(P, q + "multihead_attn", n2(x), mem, spec.heads, None, False)
-            x = x + ff(n3(x))
+            x = x + sa(n1(x))
+            x = x + ca(n2(x))
+            x = x + drop_(ff(n3(x)), sb + 5)
         else:
-            x = n1(x + _mha(P, q + "self_attn", x, x, spec.heads, bias, True))
-            x = n2(x + _mha(P, q + "multihead_attn", x, mem, spec.heads, None, False))
-            x = n3(x + ff(x))
+            x = n1(x + sa(x))
+            x = n2(x + ca(x))
+            x = n3(x + drop_(ff(x), sb + 5))
     if spec.norm_first:
         x = _layer_norm(x, P[f"{direction}.transformer.norm.weight"], P[f"{direction}.transformer.norm.bias"], 1e-5)
     return x @ P["textual.embedding.words.weight"].t() + P["textual.output.bias"]

@@ -14,9 +14,29 @@ BF16, F32 = torch.bfloat16, torch.float32
 class Recorder:
     def __init__(self):
         self.calls = []
+        self.drops = []   # (kernel, site, p) of every launch that applies a dropout mask
+
 
     def names(self):
         return [c if isinstance(c, str) else c[0] for c in self.calls]
+
+
+# kernel -> (index of p, index of site, index of the pointer whose presence means the mask is applied or None), as
+# negative offsets into the C-ABI argument list (virtex_b200/ops.py::_PROTOS)
+_DROP_ARGS = {
+    "vtx_embed_fwd": (-4, -2, None), "vtx_embed_bwd": (-4, -2, None),
+    "vtx_add_ln_fwd": (-5, -3, 1),                    # the branch operand
+    "vtx_ln_bwd": (-5, -3, 7),                        # d_branch
+    "vtx_attn_fwd": (-4, -2, None), "vtx_attn_bwd": (-4, -2, None),
+    "vtx_gelu_dropout_fwd": (-4, -2, None), "vtx_gelu_dropout_bwd": (-4, -2, None),
+}
+
+
+def _record_dropout(rec, name, args):
+    if name in _DROP_ARGS:
+        ip, isite, iptr = _DROP_ARGS[name]
+        if iptr is None or args[iptr]:
+            rec.drops.append((name, int(args[isite]), float(args[ip])))
 
 
 def _check_gemm(A, B, D, M, N, K, lda=None, ldb=None, ldd=None, a_mn=0, b_mn=0, bias=None, act=0, residual=None, ldr=0,
@@ -91,6 +111,7 @@ def dry(monkeypatch):
     def fake_call(name, *args):
         assert len(args) == len(ops._PROTOS[name]), (name, len(args), len(ops._PROTOS[name]))
         rec.calls.append(name)
+        _record_dropout(rec, name, args)
 
     def fake_gemm(A, B, D, M, N, K, **kw):
         _check_gemm(A, B, D, M, N, K, **kw)
@@ -215,3 +236,30 @@ def test_masked_lm_schedule(dry):
     with pytest.raises(ValueError):
         MaskedLMModel(visual, TransformerDecoderTextualHead(spec.visual_feature_size, spec.vocab, spec.hidden, 1,
                                                             spec.heads, spec.ffn))
+
+
+# forward kernel -> (its backward kernel, the element-index space its mask is hashed over)
+_REPLAY = {"vtx_embed_fwd": ("vtx_embed_bwd", "rows"), "vtx_add_ln_fwd": ("vtx_ln_bwd", "rows"),
+           "vtx_attn_fwd": ("vtx_attn_bwd", "attention"), "vtx_gelu_dropout_fwd": ("vtx_gelu_dropout_bwd", "ffn")}
+
+
+@pytest.mark.parametrize("norm_first,bidirectional", [(False, False), (True, False), (False, True)])
+def test_dropout_site_schedule(dry, norm_first, bidirectional):
+    """Dropout masks are recomputed in backward from (seed, site, element index): every forward site must be replayed
+    exactly once in backward by the matching kernel with the same p, no two forward sites may hash the same (site,
+    index space), and eval passes p = 0 to every dropout-carrying kernel."""
+    spec = O.Spec(hidden=128, layers=2, heads=2, ffn=256, norm_first=norm_first)
+    model = _model(spec, bidirectional=bidirectional)
+    _run(model, O.synth_batch(2, seed=3, ragged=True))
+    fwd = [d for d in dry.drops if d[0] in _REPLAY]
+    bwd = [d for d in dry.drops if d[0] not in _REPLAY]
+    assert len(fwd) == (2 if bidirectional else 1) * (1 + 6 * spec.layers)
+    assert all(p == pytest.approx(0.1) for _, _, p in fwd)
+    keys = [(site, _REPLAY[name][1]) for name, site, _ in fwd]
+    assert len(set(keys)) == len(keys), sorted(keys)
+    want = sorted((_REPLAY[name][0], site, p) for name, site, p in fwd)
+    assert sorted(bwd) == want
+    # eval: the same launches, all with p = 0
+    dry.drops.clear()
+    _run(model, O.synth_batch(2, seed=3, ragged=True), training=False, backward=False)
+    assert dry.drops and all(p == 0.0 for _, _, p in dry.drops), dry.drops

@@ -44,7 +44,8 @@ def build_model(spec: O.Spec, state, dropout=0.0):
     textual = TransformerDecoderTextualHead(
         visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
         num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=dropout,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad)
+        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad,
+        mask_future_positions=spec.mask_future)
     model = VirTexModel(visual, textual)
     missing = model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
     return model.cuda()
@@ -350,33 +351,68 @@ def test_backbone_backward_relu_open_vs_fp32_oracle():
 
 
 # -------------------------------------------------------------------------------------------------------------- head
-@pytest.mark.parametrize("layers,hidden,heads,ffn,norm_first", [(1, 128, 2, 256, False), (2, 256, 4, 512, False),
-                                                                (2, 256, 4, 512, True)])
-def test_head_forward_backward_vs_oracle(layers, hidden, heads, ffn, norm_first):
+def _head_case(layers, hidden, heads, ffn, norm_first, dropout=0.0, direction="textual", mask_future=True, id=None):
+    return pytest.param(layers, hidden, heads, ffn, norm_first, dropout, direction, mask_future, id=id)
+
+
+@pytest.mark.parametrize("layers,hidden,heads,ffn,norm_first,dropout,direction,mask_future", [
+    _head_case(1, 128, 2, 256, False, id="1-128-2-256-False"),
+    _head_case(2, 256, 4, 512, False, id="2-256-4-512-False"),
+    _head_case(2, 256, 4, 512, True, id="2-256-4-512-True"),
+    # dropout 0.1 (every pretraining config): the engine's masks replayed in the oracle at the same sites
+    _head_case(2, 256, 4, 512, False, 0.1, id="2-256-4-512-False-drop"),
+    _head_case(2, 256, 4, 512, True, 0.1, id="2-256-4-512-True-drop"),
+    _head_case(1, 512, 8, 2048, False, 0.1, id="1-512-8-2048-False-drop"),
+    _head_case(1, 768, 12, 3072, False, 0.1, id="1-768-12-3072-False-drop"),
+    _head_case(2, 256, 4, 512, False, 0.1, "backward_textual", id="2-256-4-512-False-drop-backward"),
+    _head_case(1, 256, 4, 512, False, 0.1, mask_future=False, id="1-256-4-512-False-drop-maskedlm"),
+])
+def test_head_forward_backward_vs_oracle(layers, hidden, heads, ffn, norm_first, dropout, direction, mask_future):
+    """One direction of the decoder head, forward and backward, against the fp32 oracle; at dropout > 0 with the step
+    seed set once (forward and backward read the same device word) and the oracle fed the host replica of the masks
+    (tests/dropout_replica.py).  mask_future = False is the masked-LM head (key-padding-only self-attention)."""
     _need_cuda()
-    spec = O.Spec(hidden=hidden, layers=layers, heads=heads, ffn=ffn, norm_first=norm_first)
+    from tests import dropout_replica as R
+    spec = O.Spec(hidden=hidden, layers=layers, heads=heads, ffn=ffn, norm_first=norm_first, mask_future=mask_future)
     state = O.synth_state(spec, 7)
-    model = build_model(spec, state)
+    model = build_model(spec, state, dropout=dropout)
     model.train()
     eng = model.engine
     eng.prepare_weights()
+    seed = 2 ** 63 + 5
+    eng.seed.fill_(R.as_i64(seed))
+
+    def drop(x, site):
+        if x.dim() == 4:
+            sc = R.attn_scale(seed, site, *x.shape, dropout)
+        else:
+            sc = R.flat_scale(seed, site, tuple(x.shape), dropout)
+        return x * torch.from_numpy(sc).to(x.dtype)
+
     B = 5
-    batch = O.synth_batch(B, seed=4, ragged=True)
+    batch = O.synth_masked_batch(B, seed=4) if not mask_future else O.synth_batch(B, seed=4, ragged=True)
+    labels = batch["masked_labels"].cuda() if not mask_future else None
     g = torch.Generator().manual_seed(1)
     vf = torch.randn(B, 2048, 7, 7, generator=g).abs() * 0.5
     feat = vf.permute(0, 2, 3, 1).reshape(B * 49, 2048).bfloat16().cuda().contiguous()
-    tokens, lengths = batch["caption_tokens"].cuda(), batch["caption_lengths"].cuda()
+    tok_cpu = batch["noitpac_tokens" if direction == "backward_textual" else "caption_tokens"]
+    tokens, lengths = tok_cpu.cuda(), batch["caption_lengths"].cuda()
     eng.loss.zero_(); eng.count.zero_()
     mem = eng.visual_projection_forward(feat, B * 49)
-    rec = eng.head_forward("textual", mem, tokens, lengths, training=True, want_logits_f32=True)
+    rec = eng.head_forward(direction, mem, tokens, lengths, training=True, want_logits_f32=True)
     P = {k: (v.clone().requires_grad_(True) if not O.is_buffer(k) else v.clone()) for k, v in state.items()}
     vf_ref = vf.bfloat16().float().requires_grad_(True)
-    logits_ref = O.head_forward(P, vf_ref, batch["caption_tokens"], batch["caption_lengths"], spec, "textual")
+    logits_ref = O.head_forward(P, vf_ref, tok_cpu, batch["caption_lengths"], spec, direction,
+                                drop=drop if dropout > 0 else None)
     lg = rec["logits_f32"].view(B, 30, -1)
     assert (lg.cpu() - logits_ref).abs().max().item() < 0.15, (lg.cpu() - logits_ref).abs().max().item()
-    loss_ref = O.caption_loss(logits_ref, batch["caption_tokens"], 0)
-    eng.head_loss(rec, True)
-    assert abs(eng.loss[0].item() - loss_ref.item()) < 1e-3 * loss_ref.item(), (eng.loss[0].item(), loss_ref.item())
+    if mask_future:
+        loss_ref = O.caption_loss(logits_ref, tok_cpu, 0)
+    else:
+        loss_ref = O.masked_lm_loss(logits_ref, batch["masked_labels"], 0)
+    di = 0 if direction == "textual" else 1
+    eng.head_loss(rec, True, labels)
+    assert abs(eng.loss[di].item() - loss_ref.item()) < 1e-3 * loss_ref.item(), (eng.loss[di].item(), loss_ref.item())
     loss_ref.backward()
     eng.arena.grads.zero_()
     dmem = eng.ws.get("hb.dmem", (B * 49, hidden), torch.bfloat16)
@@ -386,13 +422,20 @@ def test_head_forward_backward_vs_oracle(layers, hidden, heads, ffn, norm_first)
                     hidden, 2048)
     torch.cuda.synchronize()
     bad = []
+    checked = 0
     for name in eng.arena.names:
-        if not name.startswith("textual."):
+        if not name.startswith(("textual.", "backward_textual.")):
             continue
+        if P[name].grad is None:   # the other direction's decoder: untouched by this direction's backward
+            assert name.startswith("backward_textual." if direction == "textual" else "textual.transformer."), name
+            assert not eng.G(name).any(), name
+            continue
+        checked += 1
         r, c = rel(eng.G(name), P[name].grad), cos(eng.G(name), P[name].grad)
         if not (c > 0.999 and r < 3e-2):
             bad.append((name, r, c))
     assert not bad, bad
+    assert checked >= 8 + 16 * layers, checked
     ref_dfeat = vf_ref.grad.permute(0, 2, 3, 1).reshape(B * 49, 2048)
     assert cos(dfeat, ref_dfeat) > 0.995, cos(dfeat, ref_dfeat)
 
