@@ -300,7 +300,7 @@ def _check_fused_bn_reductions(B, monkeypatch):
             worst[:] = [r, (M, N, K, kw.get("conv_mode", 0))]
 
     monkeypatch.setattr(E, "gemm", checked_gemm)
-    eng.fuse_bn_reduce, eng.fuse_bn3_min_rows = True, 0
+    eng.fuse_bn3_min_rows = 0
     feat, h, w = eng.backbone_forward(batch["image"].cuda(), training=True)
     dfeat = (torch.randn(feat.shape, generator=torch.Generator().manual_seed(0)) * 0.01).bfloat16().cuda()
     eng.arena.grads.zero_()

@@ -17,7 +17,6 @@ decoder residual stream fp32 with bf16 shadows feeding the GEMMs, logits bf16 (f
 from __future__ import annotations
 
 import math
-import os
 import struct
 from typing import Dict, List, Optional, Tuple
 
@@ -125,6 +124,12 @@ def _require_cuda(dev):
 class Engine:
     """Forward/backward of (backbone) + (forward head) + (backward head) on one GPU.  Any part may be absent."""
 
+    # BN-backward reductions (sum dz, sum dz * xhat) are accumulated by the epilogue of the GEMM that produces the
+    # gradient (bn1 / bn2 of every block, bn3 of blocks followed by an identity block) instead of a separate pass.
+    # bn3's only for the large early-layer tensors: at layer3 / layer4 sizes the longer epilogue costs about what the
+    # stand-alone pass costs.
+    fuse_bn3_min_rows = 100000
+
     def __init__(self, visual=None, textual=None, backward_textual=None, prefix_map=None, ignore_indices=None):
         self.visual, self.textual, self.backward_textual = visual, textual, backward_textual
         named: List[Tuple[str, nn.Parameter]] = []
@@ -161,11 +166,6 @@ class Engine:
         self.generation = 0  # bumped by every forward(): a backward must match the forward that filled the tape
         self._weights_fresh = False
         self._eval_bn_fresh = False  # the running-statistics scale / shift of every BN (backbone_infer's epilogues)
-        # BN-backward reductions (sum dz, sum dz * xhat) accumulated by the epilogue of the GEMM that produces the
-        # gradient (bn1 / bn2 of every block, bn3 of blocks followed by an identity block) instead of a separate pass;
-        # VTX_BNR_FUSE=0 is the measurement knob for the A/B against the standalone vtx_bn_bwd_reduce launches
-        self.fuse_bn_reduce = os.environ.get("VTX_BNR_FUSE", "1") != "0"
-        self.fuse_bn3_min_rows = int(os.environ.get("VTX_BNR_BN3_MIN_ROWS", "100000"))  # (env: measurement knob)
         self._build_backbone_plan()
 
     # ------------------------------------------------------------------------------------------------ parameters
@@ -334,6 +334,61 @@ class Engine:
         self._slab_off += n
         return t
 
+    # Route choice + launch of the convolutions that have more than one route.  backbone_forward and backbone_infer
+    # share them, so the training and eval forwards always run the same conv; `key` names the scratch buffer of the
+    # route that needs one, and `epi` is passed through to the GEMM's epilogue.
+    def _stem_conv(self, image, y0, Ho, Wo, key, **epi):
+        """conv1 (7x7, stride 2) of the fp32 NCHW image into y0 [B*Ho*Wo, 64]; returns (s2d, cols): the GEMM operand
+        the route built, and None for the other route."""
+        B, _, H, W = image.shape
+        M0 = B * Ho * Wo
+        if H % 2 == 0 and W % 4 == 0 and Ho % 8 == 0 and Wo % 16 == 0:  # the 16 x 8 TMA boxes tile the output exactly
+            # 4-tap implicit GEMM over the space-to-depth view of the image (csrc/stem_s2d.cu)
+            s2d = self.ws.get(key + "stem.s2d", (B, H // 2 + 3, W // 2 + 3, 16), BF16)
+            call("vtx_stem_s2d", image.data_ptr(), s2d.data_ptr(), B, H, W, _stream())
+            gemm(s2d, self._packed["visual.cnn.conv1.weight#s2d"], y0, M0, 64, 256, lda=64, ldb=256,
+                 conv=(B, Ho, Wo, 64), conv_mode=5, **epi)
+            return s2d, None
+        # other image sizes: im2col + plain GEMM
+        cols = self.ws.get(key + "stem.cols", (M0, 160), BF16)
+        call("vtx_stem_im2col", image.data_ptr(), cols.data_ptr(), B, H, W, 160, _stream())
+        gemm(cols, self._packed["visual.cnn.conv1.weight"], y0, M0, 64, 160, **epi)
+        return None, cols
+
+    def _conv2(self, name, a1, y, B, Hc, Wc, stride, key, **epi):
+        """3x3 conv2 (stride) of block `name`: a1 [B*Hc*Wc, planes] -> y [Mout, planes]; returns the im2col matrix
+        when that route ran, else None."""
+        Mout, planes = y.shape
+        w2 = self._packed[name + ".conv2.weight"]
+        if planes % 64 == 0:
+            # implicit GEMM: 4-D TMA boxes gather the taps (zero fill = padding); stride 2 through TMA traversal strides
+            gemm(a1, w2, y, Mout, planes, 9 * planes, lda=planes, conv=(B, Hc, Wc, planes), conv_mode=1,
+                 conv_stride=stride, **epi)
+            return None
+        cols = self.ws.get(key, (Mout, 9 * planes), BF16)
+        call("vtx_im2col3x3", a1.data_ptr(), cols.data_ptr(), B, Hc, Wc, planes, stride, _stream())
+        gemm(cols, w2, y, Mout, planes, 9 * planes, **epi)
+        return cols
+
+    def _downsample(self, name, x, y, B, Hc, Wc, stride, key, **epi):
+        """1x1 shortcut conv (stride) of block `name`: x [B*Hc*Wc, Cin] -> y [Mout, 4*planes]; returns the matrix the
+        GEMM read (x itself at stride 1, otherwise its subsampled copy), or None when the strided implicit GEMM read x
+        in place."""
+        Mout, C4 = y.shape
+        Cin = x.shape[1]
+        wd = self.W(name + ".downsample.0.weight").view(C4, Cin)
+        if stride == 1:
+            gemm(x, wd, y, Mout, C4, Cin, **epi)
+            return x
+        if Cin % 64 == 0:  # strided 1x1 conv = one-tap implicit GEMM over x (no subsampled copy)
+            gemm(x, wd, y, Mout, C4, Cin, lda=Cin, conv=(B, Hc, Wc, Cin), conv_mode=1, conv_stride=stride, conv_taps=1,
+                 **epi)
+            return None
+        xs = self.ws.get(key, (Mout, Cin), BF16)
+        call("vtx_subsample", x.data_ptr(), xs.data_ptr(), B, Hc, Wc, Cin, stride, _stream())
+        gemm(xs, wd, y, Mout, C4, Cin, **epi)
+        return xs
+
     def backbone_forward(self, image: torch.Tensor, training: bool):
         """image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, 2048]; fills the tape used by backward."""
         if not self._weights_fresh:
@@ -350,17 +405,7 @@ class Engine:
         M0 = B * Ho * Wo
         y0 = ws.get("stem.y", (M0, 64), BF16)
         st = self._slab_take(128) if training else None
-        cols = s2d = None
-        if H % 2 == 0 and W % 4 == 0 and Ho % 8 == 0 and Wo % 16 == 0:  # the 16 x 8 TMA boxes tile the output exactly
-            # 4-tap implicit GEMM over the space-to-depth view of the image (csrc/stem_s2d.cu)
-            s2d = ws.get("stem.s2d", (B, H // 2 + 3, W // 2 + 3, 16), BF16)
-            call("vtx_stem_s2d", image.data_ptr(), s2d.data_ptr(), B, H, W, s)
-            gemm(s2d, self._packed["visual.cnn.conv1.weight#s2d"], y0, M0, 64, 256, lda=64, ldb=256, stats=st,
-                 conv=(B, Ho, Wo, 64), conv_mode=5)
-        else:  # other image sizes: im2col + plain GEMM
-            cols = ws.get("stem.cols", (M0, 160), BF16)
-            call("vtx_stem_im2col", image.data_ptr(), cols.data_ptr(), B, H, W, 160, s)
-            gemm(cols, self._packed["visual.cnn.conv1.weight"], y0, M0, 64, 160, stats=st)
+        s2d, cols = self._stem_conv(image, y0, Ho, Wo, "", stats=st)
         bnp0 = self._bn_fwd(y0, "visual.cnn.bn1", M0, 64, training, st)
         Hp, Wp = (Ho - 1) // 2 + 1, (Wo - 1) // 2 + 1
         x = ws.get("stem.pool", (B * Hp * Wp, 64), BF16)
@@ -385,17 +430,7 @@ class Engine:
             # conv2 3x3 (stride)
             y2 = ws.get(name + ".y2", (Mout, planes), BF16)
             st2 = self._slab_take(2 * planes) if training else None
-            w2 = self._packed[name + ".conv2.weight"]
-            if planes % 64 == 0:
-                # implicit GEMM: 4-D TMA boxes gather the taps (zero fill = padding); stride 2 through TMA traversal strides
-                gemm(a1, w2, y2, Mout, planes, 9 * planes, lda=planes, stats=st2, conv=(B, Hc, Wc, planes), conv_mode=1,
-                     conv_stride=stride)
-                rec["cols2"] = None
-            else:
-                cols2 = ws.get(name + ".cols2", (Mout, 9 * planes), BF16)
-                call("vtx_im2col3x3", a1.data_ptr(), cols2.data_ptr(), B, Hc, Wc, planes, stride, s)
-                gemm(cols2, w2, y2, Mout, planes, 9 * planes, stats=st2)
-                rec["cols2"] = cols2
+            rec["cols2"] = self._conv2(name, a1, y2, B, Hc, Wc, stride, name + ".cols2", stats=st2)
             a2 = ws.get(name + ".a2", (Mout, planes), BF16)
             bnp2 = self._bn_act_fwd(y2, name + ".bn2", Mout, planes, training, st2, a2)
             # conv3 1x1
@@ -410,18 +445,7 @@ class Engine:
             if blk.downsample is not None:
                 yd = ws.get(name + ".yd", (Mout, C4), BF16)
                 std = self._slab_take(2 * C4) if training else None
-                wd = self.W(name + ".downsample.0.weight").view(C4, Cin)
-                if stride == 1:
-                    xs = x
-                    gemm(xs, wd, yd, Mout, C4, Cin, stats=std)
-                elif Cin % 64 == 0:
-                    xs = None  # strided 1x1 conv = one-tap implicit GEMM over x (no subsampled copy)
-                    gemm(x, wd, yd, Mout, C4, Cin, lda=Cin, stats=std, conv=(B, Hc, Wc, Cin), conv_mode=1,
-                         conv_stride=stride, conv_taps=1)
-                else:
-                    xs = ws.get(name + ".xs", (Mout, Cin), BF16)
-                    call("vtx_subsample", x.data_ptr(), xs.data_ptr(), B, Hc, Wc, Cin, stride, s)
-                    gemm(xs, wd, yd, Mout, C4, Cin, stats=std)
+                xs = self._downsample(name, x, yd, B, Hc, Wc, stride, name + ".xs", stats=std)
                 bnpd = self._bn_fwd(yd, name + ".downsample.1", Mout, C4, training, std)
                 bnp3 = self._bn_act_fwd(y3, name + ".bn3", Mout, C4, training, st3, out, res=yd, bnp_res=bnpd, mask=m3)
                 rec.update(xs=xs, yd=yd, bnpd=bnpd)
@@ -457,15 +481,7 @@ class Engine:
         Ho, Wo = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
         M0 = B * Ho * Wo
         y0 = ws.get("inf.stem.y", (M0, 64), BF16)
-        if H % 2 == 0 and W % 4 == 0 and Ho % 8 == 0 and Wo % 16 == 0:
-            s2d = ws.get("inf.stem.s2d", (B, H // 2 + 3, W // 2 + 3, 16), BF16)
-            call("vtx_stem_s2d", image.data_ptr(), s2d.data_ptr(), B, H, W, s)
-            gemm(s2d, self._packed["visual.cnn.conv1.weight#s2d"], y0, M0, 64, 256, lda=64, ldb=256,
-                 conv=(B, Ho, Wo, 64), conv_mode=5)
-        else:
-            cols = ws.get("inf.stem.cols", (M0, 160), BF16)
-            call("vtx_stem_im2col", image.data_ptr(), cols.data_ptr(), B, H, W, 160, s)
-            gemm(cols, self._packed["visual.cnn.conv1.weight"], y0, M0, 64, 160)
+        self._stem_conv(image, y0, Ho, Wo, "inf.")
         Hp, Wp = (Ho - 1) // 2 + 1, (Wo - 1) // 2 + 1
         x = ws.get("inf.x1", (B * Hp * Wp, 64), BF16)
         idx = ws.get("inf.stem.idx", (B * Hp * Wp, 64), torch.uint8)
@@ -482,28 +498,11 @@ class Engine:
             a1 = ws.get("inf.a1", (Min, planes), BF16)
             gemm(x, self.W(name + ".conv1.weight").view(planes, Cin), a1, Min, planes, Cin, act=1, **ss(name + ".bn1"))
             a2 = ws.get("inf.a2", (Mout, planes), BF16)
-            w2 = self._packed[name + ".conv2.weight"]
-            if planes % 64 == 0:
-                gemm(a1, w2, a2, Mout, planes, 9 * planes, lda=planes, conv=(B, Hc, Wc, planes), conv_mode=1,
-                     conv_stride=stride, act=1, **ss(name + ".bn2"))
-            else:
-                cols2 = ws.get("inf.cols2", (Mout, 9 * planes), BF16)
-                call("vtx_im2col3x3", a1.data_ptr(), cols2.data_ptr(), B, Hc, Wc, planes, stride, s)
-                gemm(cols2, w2, a2, Mout, planes, 9 * planes, act=1, **ss(name + ".bn2"))
+            self._conv2(name, a1, a2, B, Hc, Wc, stride, "inf.cols2", act=1, **ss(name + ".bn2"))
             shortcut = x
             if blk.downsample is not None:
                 shortcut = ws.get("inf.shortcut", (Mout, C4), BF16)
-                wd = self.W(name + ".downsample.0.weight").view(C4, Cin)
-                sd = ss(name + ".downsample.1")
-                if stride == 1:
-                    gemm(x, wd, shortcut, Mout, C4, Cin, **sd)
-                elif Cin % 64 == 0:
-                    gemm(x, wd, shortcut, Mout, C4, Cin, lda=Cin, conv=(B, Hc, Wc, Cin), conv_mode=1, conv_stride=stride,
-                         conv_taps=1, **sd)
-                else:
-                    xs = ws.get("inf.xs", (Mout, Cin), BF16)
-                    call("vtx_subsample", x.data_ptr(), xs.data_ptr(), B, Hc, Wc, Cin, stride, s)
-                    gemm(xs, wd, shortcut, Mout, C4, Cin, **sd)
+                self._downsample(name, x, shortcut, B, Hc, Wc, stride, "inf.xs", **ss(name + ".downsample.1"))
             out = ws.get(f"inf.x{bi & 1}", (Mout, C4), BF16)
             gemm(a2, self.W(name + ".conv3.weight").view(C4, planes), out, Mout, C4, planes, residual=shortcut, act=1,
                  **ss(name + ".bn3"))
@@ -560,7 +559,6 @@ class Engine:
         self._dwp_flat.zero_()
         stem_s2d = tape["stem"]["s2d"] is not None
         blocks = tape["blocks"]
-        fuse = self.fuse_bn_reduce
         sums3 = None  # bn3 sums of the current block when the GEMM that produced dOut already accumulated them
         for bi in range(len(blocks) - 1, -1, -1):
             rec = blocks[bi]
@@ -589,9 +587,9 @@ class Engine:
             # ---- conv3 (1x1): wgrad + dgrad; the dgrad epilogue accumulates bn2's backward sums (ReLU mask from y2)
             self._wgrad(dy3, rec["a2"], self.G(name + ".conv3.weight"), C4, planes, Mout)
             da2 = ws.get("bwd.da2", (Mout, planes), BF16)
-            sums2 = self._slab_take(2 * planes) if fuse else None
+            sums2 = self._slab_take(2 * planes)
             gemm(dy3, self.W(name + ".conv3.weight").view(C4, planes), da2, Mout, planes, C4, b_mn=1,
-                 bnr=(rec["y2"], rec["bnp2"], sums2, None) if fuse else None)
+                 bnr=(rec["y2"], rec["bnp2"], sums2, None))
             # ---- bn2 + ReLU backward
             dy2 = ws.get("bwd.dy2", (Mout, planes), BF16)
             self._bn_bwd(da2, None, rec["y2"], rec["bnp2"], name + ".bn2", Mout, planes, dy2, mask_from_y=1, sums=sums2)
@@ -609,12 +607,11 @@ class Engine:
                     sk = ops.split_k_for(tiles, (Mout + 63) // 64)
                     gemm(dy2, rec["a1"], dwp, planes, 9 * planes, Mout, atomic=True, split_k=sk, lda=planes,
                          ldb=planes, conv=(B, Hc, Wc, planes), conv_mode=2, out_f32=True, conv_stride=stride)
-                if fuse and stride in (1, 2):
+                if stride in (1, 2):
                     sums1 = self._slab_take(2 * planes)  # bn1's backward sums, accumulated by the conv2-dgrad epilogue(s)
                 if stride == 1:
                     gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Min, planes, 9 * planes, lda=planes,
-                         conv=(B, Hc, Wc, planes), conv_mode=1,
-                         bnr=(rec["y1"], rec["bnp1"], sums1, None) if fuse else None)
+                         conv=(B, Hc, Wc, planes), conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
                 elif stride == 2:
                     # strided dgrad as four implicit GEMMs, one per parity class (ph, pw) of the input position: row
                     # 2i+ph of da1 gathers dy rows i+a, a < 1+ph, through kernel rows ph+1-2a (same along w); each class
@@ -631,7 +628,7 @@ class Engine:
                                  th * tw * planes, lda=planes, conv=(B, Hn, Wn, planes), conv_mode=1, tap_grid=(th, tw, 0),
                                  d_ptr=da1.data_ptr() + voff,
                                  out_view=(Hs, Ws, 2 * planes, 2 * Wc * planes, Hc * Wc * planes),
-                                 bnr=(rec["y1"], rec["bnp1"], sums1, None, rec["y1"].data_ptr() + voff) if fuse else None)
+                                 bnr=(rec["y1"], rec["bnp1"], sums1, None, rec["y1"].data_ptr() + voff))
                 else:  # other strides: per-tap gradients by a plain GEMM, scattered back by col2im
                     dcols = ws.get("bwd.dcols", (Mout, 9 * planes), BF16)
                     gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * planes, planes, b_mn=1)
@@ -676,9 +673,7 @@ class Engine:
                 # sums (ReLU bit mask m3 of THAT block) are accumulated here, over the staged dx tiles
                 prev = blocks[bi - 1] if bi > 0 else None
                 bnr3 = None
-                # (only for the large early-layer tensors: at layer3 / layer4 sizes the longer epilogue costs about what
-                # the stand-alone pass costs)
-                if fuse and prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
+                if prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
                     sums3 = self._slab_take(2 * Cin)
                     bnr3 = (prev["y3"], prev["bnp3"], sums3, prev["m3"])
                 gemm(dy1, w1, dx, Min, Cin, planes, b_mn=1, residual=dOut, residual_mask=rec["m3"], bnr=bnr3)
@@ -718,18 +713,17 @@ class Engine:
         B, T = tokens.shape
         M, H, Fd, V, A = B * T, mod.hidden_size, mod.feedforward_size, mod.vocab_size, mod.attention_heads
         S = mem.shape[0]
-        Sk = S // B
         p = float(mod.dropout) if training else 0.0
         d = direction
         di = 0 if d == "textual" else 1
         # self-attention mask: 1 = future + key padding (captioning), 2 = key padding only (masked language modelling)
-        self._mask_mode = mm = 1 if mod.mask_future_positions else 2
+        mm = 1 if mod.mask_future_positions else 2
         s = _stream()
         ws = self.ws
         seed = self.seed.data_ptr()
         site = di * 1000
-        rec = dict(direction=d, B=B, T=T, M=M, S=S, Sk=Sk, p=p, layers=[], tokens=tokens, lengths=lengths, mem=mem,
-                   mask_mode=mm)
+        rec = dict(direction=d, B=B, T=T, M=M, S=S, Sk=S // B, H=H, A=A, Fd=Fd, p=p, layers=[], tokens=tokens,
+                   lengths=lengths, mem=mem, mask_mode=mm)
         emb = "textual.embedding."
         z0 = ws.get(d + ".z0", (M, H), F32)
         st0 = ws.get(d + ".st0", (M, 2), F32)
@@ -741,60 +735,30 @@ class Engine:
              M, T, H, self.pad, 1e-8, p, seed, site, s)
         rec.update(z0=z0, st0=st0)
         for l in range(mod.num_layers):
-            q = f"{d}.transformer.layers.{l}."
             k = f"{d}.L{l}."
-            sb = site + 10 * (l + 1)
-            if mod.norm_first:
-                x = self._prenorm_layer_forward(rec, q, k, sb, x, mem, lengths, p, B, T, A, H, Fd, S, Sk)
-                continue
-            lr = dict(q=q, x_in=x, x_inb=xb)
-            # self-attention block
-            qkv = ws.get(k + "qkv", (M, 3 * H), BF16)
-            gemm(xb, self.W(q + "self_attn.in_proj_weight"), qkv, M, 3 * H, H, bias=self.P(q + "self_attn.in_proj_bias"))
-            o_s = ws.get(k + "o_s", (M, H), BF16)
-            lse_s = ws.get(k + "lse_s", (B * A * 32,), F32)
-            e = qkv.element_size()
-            call("vtx_attn_fwd", qkv.data_ptr(), 3 * H, qkv.data_ptr() + H * e, 3 * H, qkv.data_ptr() + 2 * H * e,
-                 3 * H, o_s.data_ptr(), H, lse_s.data_ptr(), B, A, T, T, lengths.data_ptr(), mm, p, seed, sb + 0, s)
+            lr = dict(q=f"{d}.transformer.layers.{l}.", k=k, sb=site + 10 * (l + 1))
             pr = ws.get(k + "proj", (M, H), BF16)
-            gemm(o_s, self.W(q + "self_attn.out_proj.weight"), pr, M, H, H, bias=self.P(q + "self_attn.out_proj.bias"))
-            z1, st1 = ws.get(k + "z1", (M, H), F32), ws.get(k + "st1", (M, 2), F32)
-            x1, x1b = ws.get(k + "x1", (M, H), F32), ws.get(k + "x1b", (M, H), BF16)
-            call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), self.P(q + "norm1.weight").data_ptr(),
-                 self.P(q + "norm1.bias").data_ptr(), z1.data_ptr(), st1.data_ptr(), x1.data_ptr(), x1b.data_ptr(), M,
-                 H, 1e-5, p, seed, sb + 1, 1, s)
-            # cross-attention block
-            wc, bc = self.W(q + "multihead_attn.in_proj_weight"), self.P(q + "multihead_attn.in_proj_bias")
-            qc = ws.get(k + "qc", (M, H), BF16)
-            gemm(x1b, wc[:H], qc, M, H, H, bias=bc[:H])
-            kv = ws.get(k + "kv", (S, 2 * H), BF16)
-            gemm(mem, wc[H:], kv, S, 2 * H, H, bias=bc[H:])
-            o_c = ws.get(k + "o_c", (M, H), BF16)
-            lse_c = ws.get(k + "lse_c", (B * A * 32,), F32)
-            call("vtx_attn_fwd", qc.data_ptr(), H, kv.data_ptr(), 2 * H, kv.data_ptr() + H * e, 2 * H, o_c.data_ptr(),
-                 H, lse_c.data_ptr(), B, A, T, Sk, 0, 0, p, seed, sb + 2, s)
-            gemm(o_c, self.W(q + "multihead_attn.out_proj.weight"), pr, M, H, H,
-                 bias=self.P(q + "multihead_attn.out_proj.bias"))
-            z2, st2 = ws.get(k + "z2", (M, H), F32), ws.get(k + "st2", (M, 2), F32)
-            x2, x2b = ws.get(k + "x2", (M, H), F32), ws.get(k + "x2b", (M, H), BF16)
-            call("vtx_add_ln_fwd", x1.data_ptr(), pr.data_ptr(), self.P(q + "norm2.weight").data_ptr(),
-                 self.P(q + "norm2.bias").data_ptr(), z2.data_ptr(), st2.data_ptr(), x2.data_ptr(), x2b.data_ptr(), M,
-                 H, 1e-5, p, seed, sb + 3, 1, s)
-            # feed-forward block
-            u = ws.get(k + "u", (M, Fd), BF16)
-            gemm(x2b, self.W(q + "linear1.weight"), u, M, Fd, H, bias=self.P(q + "linear1.bias"))
-            h = ws.get(k + "h", (M, Fd), BF16)
-            call("vtx_gelu_dropout_fwd", u.data_ptr(), h.data_ptr(), M * Fd, p, seed, sb + 4, s)
-            gemm(h, self.W(q + "linear2.weight"), pr, M, H, Fd, bias=self.P(q + "linear2.bias"))
-            z3, st3 = ws.get(k + "z3", (M, H), F32), ws.get(k + "st3", (M, 2), F32)
-            x3, x3b = ws.get(k + "x3", (M, H), F32), ws.get(k + "x3b", (M, H), BF16)
-            call("vtx_add_ln_fwd", x2.data_ptr(), pr.data_ptr(), self.P(q + "norm3.weight").data_ptr(),
-                 self.P(q + "norm3.bias").data_ptr(), z3.data_ptr(), st3.data_ptr(), x3.data_ptr(), x3b.data_ptr(), M,
-                 H, 1e-5, p, seed, sb + 5, 1, s)
-            lr.update(qkv=qkv, o_s=o_s, lse_s=lse_s, z1=z1, st1=st1, x1b=x1b, qc=qc, kv=kv, o_c=o_c, lse_c=lse_c,
-                      z2=z2, st2=st2, x2b=x2b, u=u, h=h, z3=z3, st3=st3, sb=sb)
+            for i, sublayer in enumerate((self._self_attn_fwd, self._cross_attn_fwd, self._ffn_fwd), 1):
+                norm = f"{lr['q']}norm{i}."
+                w, b = self.P(norm + "weight").data_ptr(), self.P(norm + "bias").data_ptr()
+                z, st = ws.get(f"{k}z{i}", (M, H), F32), ws.get(f"{k}st{i}", (M, 2), F32)
+                xo = ws.get(f"{k}x{i}", (M, H), F32)
+                site_i = lr["sb"] + 2 * i - 1  # the branch's dropout before the residual add
+                if mod.norm_first:  # x + dropout(f(LN(x))) (torch/nn/modules/transformer.py:1131-1143)
+                    xb = ws.get(f"{k}n{i}b", (M, H), BF16)
+                    call("vtx_add_ln_fwd", x.data_ptr(), 0, w, b, z.data_ptr(), st.data_ptr(), 0, xb.data_ptr(), M, H,
+                         1e-5, 0.0, seed, 0, 1, s)
+                    sublayer(rec, lr, xb, pr)
+                    call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), 0, 0, xo.data_ptr(), 0, 0, 0, M, H, 0.0, p,
+                         seed, site_i, 0, s)
+                else:  # LN(x + dropout(f(x))), with a bf16 shadow of the result for the next sublayer's GEMMs
+                    sublayer(rec, lr, xb, pr)
+                    xb = ws.get(f"{k}x{i}b", (M, H), BF16)
+                    call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), w, b, z.data_ptr(), st.data_ptr(),
+                         xo.data_ptr(), xb.data_ptr(), M, H, 1e-5, p, seed, site_i, 1, s)
+                x = xo
+                lr.update({f"z{i}": z, f"st{i}": st})
             rec["layers"].append(lr)
-            x, xb = x3, x3b
         if mod.norm_first:  # final LayerNorm of pre-norm decoders (textual_heads.py:192-193)
             qn = f"{d}.transformer.norm."
             zf, stf = ws.get(d + ".zf", (M, H), F32), ws.get(d + ".stf", (M, 2), F32)
@@ -815,117 +779,87 @@ class Engine:
         rec["logits"] = logits
         return rec
 
-    def _prenorm_layer_forward(self, rec, q, k, sb, x, mem, lengths, p, B, T, A, H, Fd, S, Sk):
-        """x + f(LN(x)) for the three blocks (torch/nn/modules/transformer.py:1131-1143); returns the new fp32 x."""
-        s, ws, seed = _stream(), self.ws, self.seed.data_ptr()
-        M = B * T
-        e = 2
-        lr = dict(q=q, sb=sb, x0=x)
+    def _attn_fwd(self, rec, q, k, v, o, lse, Tk, lengths, mask_mode, site):
+        """Multi-head attention of the T query rows of each caption over its Tk key rows.  q, k, v, o: row-major views
+        (column slices of a fused projection are fine) whose leading dimensions are their row strides."""
+        call("vtx_attn_fwd", q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+             o.data_ptr(), o.stride(0), lse.data_ptr(), rec["B"], rec["A"], rec["T"], Tk, _p(lengths), mask_mode,
+             rec["p"], self.seed.data_ptr(), site, _stream())
 
-        def norm(name, xin, tag):
-            z, st = ws.get(k + "z" + tag, (M, H), F32), ws.get(k + "st" + tag, (M, 2), F32)
-            nb = ws.get(k + "n" + tag + "b", (M, H), BF16)
-            call("vtx_add_ln_fwd", xin.data_ptr(), 0, self.P(q + name + ".weight").data_ptr(),
-                 self.P(q + name + ".bias").data_ptr(), z.data_ptr(), st.data_ptr(), 0, nb.data_ptr(), M, H, 1e-5, 0.0,
-                 seed, 0, 1, s)
-            return z, st, nb
+    def _attn_bwd(self, rec, q, k, v, do, lse, dq, dk, dv, Tk, lengths, mask_mode, site):
+        """Backward of _attn_fwd: dq, dk, dv (views as q, k, v) from do and the forward's log-sum-exp rows."""
+        call("vtx_attn_bwd", q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+             do.data_ptr(), do.stride(0), lse.data_ptr(), dq.data_ptr(), dq.stride(0), dk.data_ptr(), dk.stride(0),
+             dv.data_ptr(), dv.stride(0), rec["B"], rec["A"], rec["T"], Tk, _p(lengths), mask_mode, rec["p"],
+             self.seed.data_ptr(), site, _stream())
 
-        def residual(xin, branch, tag, site):
-            xo = ws.get(k + "x" + tag, (M, H), F32)
-            call("vtx_add_ln_fwd", xin.data_ptr(), branch.data_ptr(), 0, 0, xo.data_ptr(), 0, 0, 0, M, H, 0.0, p, seed,
-                 site, 0, s)
-            return xo
+    # The three sublayers of a decoder layer.  Each forward reads the bf16 [M, H] input `x` (post-norm: the previous
+    # LayerNorm's bf16 shadow; pre-norm: the sublayer's own LayerNorm output), writes its branch output to `out` and
+    # keeps what its backward needs in the layer tape `lr`.  Each backward goes from the bf16 branch gradient `dy` to
+    # the gradient `dx` of that input and accumulates the parameter gradients.
+    def _self_attn_fwd(self, rec, lr, x, out):
+        M, H, q, k = rec["M"], rec["H"], lr["q"] + "self_attn.", lr["k"]
+        qkv = self.ws.get(k + "qkv", (M, 3 * H), BF16)
+        gemm(x, self.W(q + "in_proj_weight"), qkv, M, 3 * H, H, bias=self.P(q + "in_proj_bias"))
+        o = self.ws.get(k + "o_s", (M, H), BF16)
+        lse = self.ws.get(k + "lse_s", (rec["B"] * rec["A"] * 32,), F32)
+        self._attn_fwd(rec, *qkv.split(H, 1), o, lse, rec["T"], rec["lengths"], rec["mask_mode"], lr["sb"])
+        gemm(o, self.W(q + "out_proj.weight"), out, M, H, H, bias=self.P(q + "out_proj.bias"))
+        lr.update(x_s=x, qkv=qkv, o_s=o, lse_s=lse)
 
-        pr = ws.get(k + "proj", (M, H), BF16)
-        # self attention
-        z1, st1, n1b = norm("norm1", x, "1")
-        qkv = ws.get(k + "qkv", (M, 3 * H), BF16)
-        gemm(n1b, self.W(q + "self_attn.in_proj_weight"), qkv, M, 3 * H, H, bias=self.P(q + "self_attn.in_proj_bias"))
-        o_s = ws.get(k + "o_s", (M, H), BF16)
-        lse_s = ws.get(k + "lse_s", (B * A * 32,), F32)
-        call("vtx_attn_fwd", qkv.data_ptr(), 3 * H, qkv.data_ptr() + H * e, 3 * H, qkv.data_ptr() + 2 * H * e, 3 * H,
-             o_s.data_ptr(), H, lse_s.data_ptr(), B, A, T, T, lengths.data_ptr(), rec["mask_mode"], p, seed, sb + 0, s)
-        gemm(o_s, self.W(q + "self_attn.out_proj.weight"), pr, M, H, H, bias=self.P(q + "self_attn.out_proj.bias"))
-        x1 = residual(x, pr, "1", sb + 1)
-        # cross attention
-        z2, st2, n2b = norm("norm2", x1, "2")
-        wc, bc = self.W(q + "multihead_attn.in_proj_weight"), self.P(q + "multihead_attn.in_proj_bias")
-        qc = ws.get(k + "qc", (M, H), BF16)
-        gemm(n2b, wc[:H], qc, M, H, H, bias=bc[:H])
-        kv = ws.get(k + "kv", (S, 2 * H), BF16)
-        gemm(mem, wc[H:], kv, S, 2 * H, H, bias=bc[H:])
-        o_c = ws.get(k + "o_c", (M, H), BF16)
-        lse_c = ws.get(k + "lse_c", (B * A * 32,), F32)
-        call("vtx_attn_fwd", qc.data_ptr(), H, kv.data_ptr(), 2 * H, kv.data_ptr() + H * e, 2 * H, o_c.data_ptr(), H,
-             lse_c.data_ptr(), B, A, T, Sk, 0, 0, p, seed, sb + 2, s)
-        gemm(o_c, self.W(q + "multihead_attn.out_proj.weight"), pr, M, H, H,
-             bias=self.P(q + "multihead_attn.out_proj.bias"))
-        x2 = residual(x1, pr, "2", sb + 3)
-        # feed forward
-        z3, st3, n3b = norm("norm3", x2, "3")
-        u = ws.get(k + "u", (M, Fd), BF16)
-        gemm(n3b, self.W(q + "linear1.weight"), u, M, Fd, H, bias=self.P(q + "linear1.bias"))
-        h = ws.get(k + "h", (M, Fd), BF16)
-        call("vtx_gelu_dropout_fwd", u.data_ptr(), h.data_ptr(), M * Fd, p, seed, sb + 4, s)
-        gemm(h, self.W(q + "linear2.weight"), pr, M, H, Fd, bias=self.P(q + "linear2.bias"))
-        x3 = residual(x2, pr, "3", sb + 5)
-        lr.update(z1=z1, st1=st1, n1b=n1b, qkv=qkv, o_s=o_s, lse_s=lse_s, z2=z2, st2=st2, n2b=n2b, qc=qc, kv=kv, o_c=o_c,
-                  lse_c=lse_c, z3=z3, st3=st3, n3b=n3b, u=u, h=h)
-        rec["layers"].append(lr)
-        return x3
+    def _self_attn_bwd(self, rec, lr, dy, dx):
+        M, H, q = rec["M"], rec["H"], lr["q"] + "self_attn."
+        do = self.ws.get("hb.do", (M, H), BF16)
+        self._linear_bwd(dy, lr["o_s"], q + "out_proj.weight", q + "out_proj.bias", do, M, H, H)
+        dqkv = self.ws.get("hb.dqkv", (M, 3 * H), BF16)
+        self._attn_bwd(rec, *lr["qkv"].split(H, 1), do, lr["lse_s"], *dqkv.split(H, 1), rec["T"], rec["lengths"],
+                       rec["mask_mode"], lr["sb"])
+        self._linear_bwd(dqkv, lr["x_s"], q + "in_proj_weight", q + "in_proj_bias", dx, M, 3 * H, H)
 
-    def _prenorm_layer_backward(self, rec, lr, g, dmem, dmem_started, mod):
-        """g = dL/dx_out (fp32 [M,H], updated in place to dL/dx_in)."""
-        B, T, M, S, Sk, p = rec["B"], rec["T"], rec["M"], rec["S"], rec["Sk"], rec["p"]
-        H, Fd, A = mod.hidden_size, mod.feedforward_size, mod.attention_heads
-        s, ws, seed = _stream(), self.ws, self.seed.data_ptr()
-        q, sb = lr["q"], lr["sb"]
-        e = 2
-        dbr = ws.get("hb.dbr", (M, H), BF16)
-        dxb = ws.get("hb.dxb", (M, H), BF16)
-        do = ws.get("hb.do", (M, H), BF16)
+    def _cross_attn_fwd(self, rec, lr, x, out):
+        M, H, S, q, k = rec["M"], rec["H"], rec["S"], lr["q"] + "multihead_attn.", lr["k"]
+        w, b = self.W(q + "in_proj_weight"), self.P(q + "in_proj_bias")
+        qc = self.ws.get(k + "qc", (M, H), BF16)
+        gemm(x, w[:H], qc, M, H, H, bias=b[:H])
+        kv = self.ws.get(k + "kv", (S, 2 * H), BF16)
+        gemm(rec["mem"], w[H:], kv, S, 2 * H, H, bias=b[H:])
+        o = self.ws.get(k + "o_c", (M, H), BF16)
+        lse = self.ws.get(k + "lse_c", (rec["B"] * rec["A"] * 32,), F32)
+        self._attn_fwd(rec, qc, *kv.split(H, 1), o, lse, rec["Sk"], None, 0, lr["sb"] + 2)
+        gemm(o, self.W(q + "out_proj.weight"), out, M, H, H, bias=self.P(q + "out_proj.bias"))
+        lr.update(x_c=x, qc=qc, kv=kv, o_c=o, lse_c=lse)
 
-        def branch_grad(site):  # d(branch) = g * dropout mask (bf16); g itself keeps flowing through the skip path
-            call("vtx_ln_bwd", g.data_ptr(), 0, 0, 0, 0, 0, 0, dbr.data_ptr(), 0, 0, M, H, p, seed, site, 0, s)
-
-        def norm_bwd(name, z, st, dn):  # g += LN_backward(dn)
-            call("vtx_ln_bwd", 0, dn.data_ptr(), z.data_ptr(), st.data_ptr(), self.P(q + name + ".weight").data_ptr(),
-                 g.data_ptr(), g.data_ptr(), 0, self.G(q + name + ".weight").data_ptr(),
-                 self.G(q + name + ".bias").data_ptr(), M, H, 0.0, seed, 0, 1, s)
-
-        # feed forward
-        branch_grad(sb + 5)
-        dh = ws.get("hb.dh", (M, Fd), BF16)
-        self._linear_bwd(dbr, lr["h"], q + "linear2.weight", q + "linear2.bias", dh, M, H, Fd)
-        call("vtx_gelu_dropout_bwd", dh.data_ptr(), lr["u"].data_ptr(), dh.data_ptr(), M * Fd, p, seed, sb + 4, s)
-        self._linear_bwd(dh, lr["n3b"], q + "linear1.weight", q + "linear1.bias", dxb, M, Fd, H)
-        norm_bwd("norm3", lr["z3"], lr["st3"], dxb)
-        # cross attention
-        branch_grad(sb + 3)
-        self._linear_bwd(dbr, lr["o_c"], q + "multihead_attn.out_proj.weight", q + "multihead_attn.out_proj.bias", do,
-                         M, H, H)
-        dqc = ws.get("hb.dqc", (M, H), BF16)
-        dkv = ws.get("hb.dkv", (S, 2 * H), BF16)
-        kv = lr["kv"]
-        call("vtx_attn_bwd", lr["qc"].data_ptr(), H, kv.data_ptr(), 2 * H, kv.data_ptr() + H * e, 2 * H, do.data_ptr(),
-             H, lr["lse_c"].data_ptr(), dqc.data_ptr(), H, dkv.data_ptr(), 2 * H, dkv.data_ptr() + H * e, 2 * H, B, A, T,
-             Sk, 0, 0, p, seed, sb + 2, s)
-        wn, bn = q + "multihead_attn.in_proj_weight", q + "multihead_attn.in_proj_bias"
-        self._linear_bwd(dqc, lr["n2b"], wn, bn, dxb, M, H, H, w_rows=slice(0, H))
+    def _cross_attn_bwd(self, rec, lr, dy, dx, dmem, dmem_started):
+        """Also adds the gradient of the visual memory to dmem [S, H] (overwrites it while not dmem_started)."""
+        M, H, S, q = rec["M"], rec["H"], rec["S"], lr["q"] + "multihead_attn."
+        do = self.ws.get("hb.do", (M, H), BF16)
+        self._linear_bwd(dy, lr["o_c"], q + "out_proj.weight", q + "out_proj.bias", do, M, H, H)
+        dqc = self.ws.get("hb.dqc", (M, H), BF16)
+        dkv = self.ws.get("hb.dkv", (S, 2 * H), BF16)
+        self._attn_bwd(rec, lr["qc"], *lr["kv"].split(H, 1), do, lr["lse_c"], dqc, *dkv.split(H, 1), rec["Sk"], None, 0,
+                       lr["sb"] + 2)
+        wn, bn = q + "in_proj_weight", q + "in_proj_bias"
+        self._linear_bwd(dqc, lr["x_c"], wn, bn, dx, M, H, H, w_rows=slice(0, H))
         self._linear_bwd(dkv, rec["mem"], wn, bn, dmem, S, 2 * H, H, w_rows=slice(H, 3 * H),
                          residual=dmem if dmem_started else None)
-        norm_bwd("norm2", lr["z2"], lr["st2"], dxb)
-        # self attention
-        branch_grad(sb + 1)
-        self._linear_bwd(dbr, lr["o_s"], q + "self_attn.out_proj.weight", q + "self_attn.out_proj.bias", do, M, H, H)
-        dqkv = ws.get("hb.dqkv", (M, 3 * H), BF16)
-        qkv = lr["qkv"]
-        call("vtx_attn_bwd", qkv.data_ptr(), 3 * H, qkv.data_ptr() + H * e, 3 * H, qkv.data_ptr() + 2 * H * e, 3 * H,
-             do.data_ptr(), H, lr["lse_s"].data_ptr(), dqkv.data_ptr(), 3 * H, dqkv.data_ptr() + H * e, 3 * H,
-             dqkv.data_ptr() + 2 * H * e, 3 * H, B, A, T, T, rec["lengths"].data_ptr(), rec["mask_mode"], p, seed, sb + 0,
-             s)
-        self._linear_bwd(dqkv, lr["n1b"], q + "self_attn.in_proj_weight", q + "self_attn.in_proj_bias", dxb, M, 3 * H, H)
-        norm_bwd("norm1", lr["z1"], lr["st1"], dxb)
+
+    def _ffn_fwd(self, rec, lr, x, out):
+        M, H, Fd, q, k = rec["M"], rec["H"], rec["Fd"], lr["q"], lr["k"]
+        u = self.ws.get(k + "u", (M, Fd), BF16)
+        gemm(x, self.W(q + "linear1.weight"), u, M, Fd, H, bias=self.P(q + "linear1.bias"))
+        h = self.ws.get(k + "h", (M, Fd), BF16)
+        call("vtx_gelu_dropout_fwd", u.data_ptr(), h.data_ptr(), M * Fd, rec["p"], self.seed.data_ptr(), lr["sb"] + 4,
+             _stream())
+        gemm(h, self.W(q + "linear2.weight"), out, M, H, Fd, bias=self.P(q + "linear2.bias"))
+        lr.update(x_f=x, u=u, h=h)
+
+    def _ffn_bwd(self, rec, lr, dy, dx):
+        M, H, Fd, q = rec["M"], rec["H"], rec["Fd"], lr["q"]
+        dh = self.ws.get("hb.dh", (M, Fd), BF16)
+        self._linear_bwd(dy, lr["h"], q + "linear2.weight", q + "linear2.bias", dh, M, H, Fd)
+        call("vtx_gelu_dropout_bwd", dh.data_ptr(), lr["u"].data_ptr(), dh.data_ptr(), M * Fd, rec["p"],
+             self.seed.data_ptr(), lr["sb"] + 4, _stream())
+        self._linear_bwd(dh, lr["x_f"], q + "linear1.weight", q + "linear1.bias", dx, M, Fd, H)
 
     def head_loss(self, rec, write_grad, labels=None):
         """Token-mean cross entropy (ignore_index = pad).  labels None: next-token targets tokens[:, 1:] against
@@ -957,8 +891,8 @@ class Engine:
         Accumulates parameter gradients; adds this direction's contribution to dmem [S,H]."""
         d = rec["direction"]
         mod = self._head_modules(d)
-        B, T, M, S, Sk, p = rec["B"], rec["T"], rec["M"], rec["S"], rec["Sk"], rec["p"]
-        H, Fd, V, A = mod.hidden_size, mod.feedforward_size, mod.vocab_size, mod.attention_heads
+        T, M, H, p = rec["T"], rec["M"], rec["H"], rec["p"]
+        V = mod.vocab_size
         s = _stream()
         ws = self.ws
         seed = self.seed.data_ptr()
@@ -971,61 +905,39 @@ class Engine:
         dres_a = ws.get("hb.dres_a", (M, H), F32)
         dres_b = ws.get("hb.dres_b", (M, H), F32)
         dbr = ws.get("hb.dbr", (M, H), BF16)
-        dy_a, dy_b = None, dxb
-        e = 2
+        dy_a, dy_b = None, dxb  # gradient of the residual stream: fp32 part, bf16 part (of a bf16 shadow's reader)
         if mod.norm_first:
             qn = f"{d}.transformer.norm."
-            g = dres_a
             call("vtx_ln_bwd", 0, dxb.data_ptr(), rec["zf"].data_ptr(), rec["stf"].data_ptr(),
-                 self.P(qn + "weight").data_ptr(), 0, g.data_ptr(), 0, self.G(qn + "weight").data_ptr(),
+                 self.P(qn + "weight").data_ptr(), 0, dres_a.data_ptr(), 0, self.G(qn + "weight").data_ptr(),
                  self.G(qn + "bias").data_ptr(), M, H, 0.0, seed, 0, 1, s)
-            for l in reversed(range(mod.num_layers)):
-                self._prenorm_layer_backward(rec, rec["layers"][l], g, dmem, dmem_started, mod)
-                dmem_started = True
-            dy_a, dy_b = g, None
-        for l in (reversed(range(mod.num_layers)) if not mod.norm_first else ()):
+            dy_a, dy_b = dres_a, None
+        for l in reversed(range(mod.num_layers)):
             lr = rec["layers"][l]
-            q, sb = lr["q"], lr["sb"]
-            # LN3 / FFN
-            call("vtx_ln_bwd", _p(dy_a), _p(dy_b), lr["z3"].data_ptr(), lr["st3"].data_ptr(),
-                 self.P(q + "norm3.weight").data_ptr(), 0, dres_a.data_ptr(), dbr.data_ptr(),
-                 self.G(q + "norm3.weight").data_ptr(), self.G(q + "norm3.bias").data_ptr(), M, H, p, seed, sb + 5, 1, s)
-            dh = ws.get("hb.dh", (M, Fd), BF16)
-            self._linear_bwd(dbr, lr["h"], q + "linear2.weight", q + "linear2.bias", dh, M, H, Fd)
-            call("vtx_gelu_dropout_bwd", dh.data_ptr(), lr["u"].data_ptr(), dh.data_ptr(), M * Fd, p, seed, sb + 4, s)
-            self._linear_bwd(dh, lr["x2b"], q + "linear1.weight", q + "linear1.bias", dxb, M, Fd, H)
-            # LN2 / cross attention
-            call("vtx_ln_bwd", dres_a.data_ptr(), dxb.data_ptr(), lr["z2"].data_ptr(), lr["st2"].data_ptr(),
-                 self.P(q + "norm2.weight").data_ptr(), 0, dres_b.data_ptr(), dbr.data_ptr(),
-                 self.G(q + "norm2.weight").data_ptr(), self.G(q + "norm2.bias").data_ptr(), M, H, p, seed, sb + 3, 1, s)
-            do = ws.get("hb.do", (M, H), BF16)
-            self._linear_bwd(dbr, lr["o_c"], q + "multihead_attn.out_proj.weight", q + "multihead_attn.out_proj.bias",
-                             do, M, H, H)
-            dqc = ws.get("hb.dqc", (M, H), BF16)
-            dkv = ws.get("hb.dkv", (S, 2 * H), BF16)
-            kv = lr["kv"]
-            call("vtx_attn_bwd", lr["qc"].data_ptr(), H, kv.data_ptr(), 2 * H, kv.data_ptr() + H * e, 2 * H,
-                 do.data_ptr(), H, lr["lse_c"].data_ptr(), dqc.data_ptr(), H, dkv.data_ptr(), 2 * H,
-                 dkv.data_ptr() + H * e, 2 * H, B, A, T, Sk, 0, 0, p, seed, sb + 2, s)
-            wn, bn = q + "multihead_attn.in_proj_weight", q + "multihead_attn.in_proj_bias"
-            self._linear_bwd(dqc, lr["x1b"], wn, bn, dxb, M, H, H, w_rows=slice(0, H))
-            self._linear_bwd(dkv, rec["mem"], wn, bn, dmem, S, 2 * H, H, w_rows=slice(H, 3 * H),
-                             residual=dmem if dmem_started else None)
-            dmem_started = True
-            # LN1 / self attention
-            call("vtx_ln_bwd", dres_b.data_ptr(), dxb.data_ptr(), lr["z1"].data_ptr(), lr["st1"].data_ptr(),
-                 self.P(q + "norm1.weight").data_ptr(), 0, dres_a.data_ptr(), dbr.data_ptr(),
-                 self.G(q + "norm1.weight").data_ptr(), self.G(q + "norm1.bias").data_ptr(), M, H, p, seed, sb + 1, 1, s)
-            self._linear_bwd(dbr, lr["o_s"], q + "self_attn.out_proj.weight", q + "self_attn.out_proj.bias", do, M, H, H)
-            dqkv = ws.get("hb.dqkv", (M, 3 * H), BF16)
-            qkv = lr["qkv"]
-            call("vtx_attn_bwd", qkv.data_ptr(), 3 * H, qkv.data_ptr() + H * e, 3 * H, qkv.data_ptr() + 2 * H * e,
-                 3 * H, do.data_ptr(), H, lr["lse_s"].data_ptr(), dqkv.data_ptr(), 3 * H, dqkv.data_ptr() + H * e,
-                 3 * H, dqkv.data_ptr() + 2 * H * e, 3 * H, B, A, T, T, rec["lengths"].data_ptr(), rec["mask_mode"], p, seed,
-                 sb + 0, s)
-            self._linear_bwd(dqkv, lr["x_inb"], q + "self_attn.in_proj_weight", q + "self_attn.in_proj_bias", dxb, M,
-                             3 * H, H)
-            dy_a, dy_b = dres_a, dxb
+            for i in (3, 2, 1):
+                norm = f"{lr['q']}norm{i}."
+                w, dw, db = (self.P(norm + "weight").data_ptr(), self.G(norm + "weight").data_ptr(),
+                             self.G(norm + "bias").data_ptr())
+                z, st = lr[f"z{i}"].data_ptr(), lr[f"st{i}"].data_ptr()
+                site_i = lr["sb"] + 2 * i - 1
+                if mod.norm_first:  # d(branch) = g * dropout mask (bf16); g itself keeps flowing through the skip path
+                    call("vtx_ln_bwd", dres_a.data_ptr(), 0, 0, 0, 0, 0, 0, dbr.data_ptr(), 0, 0, M, H, p, seed, site_i,
+                         0, s)
+                else:  # through LN(x + dropout(branch)): fp32 gradient of x, bf16 gradient of the branch
+                    dres = dres_b if i == 2 else dres_a
+                    call("vtx_ln_bwd", _p(dy_a), _p(dy_b), z, st, w, 0, dres.data_ptr(), dbr.data_ptr(), dw, db, M, H,
+                         p, seed, site_i, 1, s)
+                    dy_a, dy_b = dres, dxb
+                if i == 3:
+                    self._ffn_bwd(rec, lr, dbr, dxb)
+                elif i == 2:
+                    self._cross_attn_bwd(rec, lr, dbr, dxb, dmem, dmem_started)
+                    dmem_started = True
+                else:
+                    self._self_attn_bwd(rec, lr, dbr, dxb)
+                if mod.norm_first:  # g += LN_backward(dxb)
+                    call("vtx_ln_bwd", 0, dxb.data_ptr(), z, st, w, dres_a.data_ptr(), dres_a.data_ptr(), 0, dw, db, M,
+                         H, 0.0, seed, 0, 1, s)
         emb = "textual.embedding."
         di = 0 if d == "textual" else 1
         call("vtx_embed_bwd", _p(dy_a), _p(dy_b), rec["tokens"].data_ptr(), rec["z0"].data_ptr(),
