@@ -148,10 +148,11 @@ int vtx_bn_finalize(const float* stats, float count, const float* gamma, const f
                     float* running_var, int64_t* num_batches_tracked, float momentum, float eps, int training,
                     float* bnp, int C, void* stream);
 /* out = act(y*scale + shift [+ res | + res*scale_r + shift_r]).  relu_mask (optional, relu only): uint8 [M, C/8], bit j
-   of byte (m, g) = [pre-activation of channel 8g + j > 0] -- all that BN backward needs of `out` (1/16 of its bytes) */
+   of byte (m, g) = [pre-activation of channel 8g + j > 0] -- all that BN backward needs of `out` (1/16 of its bytes).
+   C/8 must divide 256 (C = 8, 16, 32, ..., 2048); any other C is rejected with VTX_EINVAL. */
 int vtx_bn_act(const void* y, const float* bnp, const void* res, const float* bnp_res, void* out, uint8_t* relu_mask,
                int64_t M, int C, int relu, void* stream);
-/* vtx_bn_finalize + vtx_bn_act fused into one launch */
+/* vtx_bn_finalize + vtx_bn_act fused into one launch; C/8 must divide 256, as for vtx_bn_act */
 int vtx_bn_finalize_act(const float* stats, float count, const float* gamma, const float* beta, float* running_mean,
                         float* running_var, int64_t* num_batches_tracked, float momentum, float eps, int training,
                         float* bnp, const void* y, const void* res, const float* bnp_res, void* out, uint8_t* relu_mask,
@@ -162,7 +163,9 @@ int vtx_maxpool_bwd(const void* dpool, const uint8_t* idx, void* da, int N, int 
 /* BN backward in three steps: per-channel sums of dz and dz*xhat (dz = dA*[relu_mask bit]); coefficients + dgamma/dbeta;
    dy = scale*(dz - mean(dz) - xhat*mean(dz*xhat)).  A second BN sharing dz (downsample branch) rides along.
    relu_mask: the uint8 bit mask written by vtx_bn_act / vtx_bn_finalize_act, or NULL;
-   relu_mask == NULL && mask_from_y: the ReLU mask is recomputed as [y*scale + shift > 0] instead of being read. */
+   relu_mask == NULL && mask_from_y: the ReLU mask is recomputed as [y*scale + shift > 0] instead of being read.
+   vtx_bn_bwd_reduce takes any C % 8 == 0 with C/8 <= 256; vtx_bn_bwd_apply and vtx_bn_bwd_finalize_apply need C/8 to
+   divide 256 (C = 8, 16, 32, ..., 2048) and reject any other C with VTX_EINVAL. */
 int vtx_bn_bwd_reduce(const void* dA, const uint8_t* relu_mask, const void* y, const float* bnp, const void* y2,
                       const float* bnp2, float* sums, float* sums2, int64_t M, int C, int mask_from_y,
                       void* stream);

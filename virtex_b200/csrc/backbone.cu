@@ -1045,6 +1045,10 @@ using namespace vtx;
 #define STREAM reinterpret_cast<cudaStream_t>(stream)
 #define REQ(cond, msg) \
   if (!(cond)) return set_error(VTX_EINVAL, "%s: %s", __func__, msg)
+// bn_act_kernel and bn_bwd_apply_kernel keep a thread's 8 channels of BN parameters in registers for the whole
+// grid-stride loop.  That is only right when the channel group of element i, i % (C/8), does not change when i steps by
+// the grid stride (a multiple of 256): C/8 must divide 256.
+static const char kBnGroupMsg[] = "needs 256 % (C / 8) == 0, i.e. C in {8, 16, 32, ..., 2048}";
 
 extern "C" int vtx_stem_im2col(const float* img, void* cols, int N, int H, int W, int ldc, void* stream) {
   REQ(img && cols && ldc >= 152 && ldc % 8 == 0, "bad arguments");
@@ -1118,6 +1122,7 @@ extern "C" int vtx_bn_finalize(const float* stats, float count, const float* gam
 extern "C" int vtx_bn_act(const void* y, const float* bnp, const void* res, const float* bnp_res, void* out,
                           uint8_t* relu_mask, int64_t M, int C, int relu, void* stream) {
   REQ(y && bnp && out && C % 8 == 0, "bad arguments");
+  REQ(C >= 8 && 256 % (C / 8) == 0, kBnGroupMsg);
   BnFwdFold f;
   memset(&f, 0, sizeof(f));
   if (res == nullptr)
@@ -1134,8 +1139,8 @@ extern "C" int vtx_bn_finalize_act(const float* stats, float count, const float*
                                    float* rvar, int64_t* nbt, float momentum, float eps, int training, float* bnp,
                                    const void* y, const void* res, const float* bnp_res, void* out, uint8_t* relu_mask,
                                    int64_t M, int C, int relu, void* stream) {
-  REQ(y && bnp && out && gamma && beta && rmean && rvar && C % 8 == 0 && C / 8 <= 256 && (stats || !training),
-      "bad arguments");
+  REQ(y && bnp && out && gamma && beta && rmean && rvar && C % 8 == 0 && (stats || !training), "bad arguments");
+  REQ(C >= 8 && 256 % (C / 8) == 0, kBnGroupMsg);
   BnFwdFold f;
   f.stats = stats; f.gamma = gamma; f.beta = beta; f.rmean = rmean; f.rvar = rvar; f.nbt = (long long*)nbt;
   f.count = count; f.momentum = momentum; f.eps = eps; f.training = training;
@@ -1239,6 +1244,7 @@ extern "C" int vtx_bn_bwd_apply(const void* dA, const uint8_t* a, const void* y,
                                 void* dy, const void* y2, const float* bnp2, const float* coef2, void* dy2,
                                 void* dz_out, int64_t M, int C, int mask_from_y, void* stream) {
   REQ(dA && y && bnp && coef && dy && C % 8 == 0, "bad arguments");
+  REQ(C >= 8 && 256 % (C / 8) == 0, kBnGroupMsg);
   if (y2 != nullptr) REQ(bnp2 && coef2 && dy2, "second BN needs bnp2/coef2/dy2");
   BnBwdFold f;
   memset(&f, 0, sizeof(f));
@@ -1249,7 +1255,8 @@ extern "C" int vtx_bn_bwd_finalize_apply(const float* sums, const float* sums2, 
                                          float* dgamma2, float* dbeta2, const void* dA, const uint8_t* a, const void* y,
                                          const float* bnp, void* dy, const void* y2, const float* bnp2, void* dy2,
                                          void* dz_out, int64_t M, int C, int mask_from_y, void* stream) {
-  REQ(sums && dA && y && bnp && dy && C % 8 == 0 && C / 8 <= 256, "bad arguments");
+  REQ(sums && dA && y && bnp && dy && C % 8 == 0, "bad arguments");
+  REQ(C >= 8 && 256 % (C / 8) == 0, kBnGroupMsg);
   if (y2 != nullptr) REQ(bnp2 && sums2 && dy2, "second BN needs bnp2/sums2/dy2");
   BnBwdFold f;
   f.sums = sums; f.sums2 = sums2; f.dgamma = dgamma; f.dbeta = dbeta; f.dgamma2 = dgamma2; f.dbeta2 = dbeta2;
