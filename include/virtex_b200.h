@@ -263,6 +263,41 @@ int vtx_khot_xent(void* logits, int64_t ldl, const int64_t* labels, int64_t ldla
 int vtx_topk_rows(const float* X, int64_t ld, int M, int N, int k, int64_t* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Incremental beam-search decoding (csrc/decode.cu): AutoRegressiveBeamSearch over CaptioningModel.decoding_step
+ * (virtex/utils/beam_search.py:52-238, virtex/models/captioning.py:144-213) with a key/value cache instead of a full
+ * recompute per step.  Step tables are step-major: pred int64 [steps, R] and index int32 [steps, R], R = B * beam, so
+ * that step t of every row is one contiguous row (the token input of the next step's vtx_embed_fwd with T = 1).
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define VTX_DECODE_MAX_KEYS 64
+/* One query per row, head_dim 64, 1 <= Tk <= VTX_DECODE_MAX_KEYS keys, no mask, no dropout.  Query row m = b * group + g
+   (g < group) of head h attends over the Tk keys of block b:
+       key j  = k + blk * ldb + j * ldkv + 64 h,   value j = v + blk * ldb + j * ldkv + 64 h,
+       blk    = b, or kv_index[j * ld_index + b] when kv_index != NULL (needs group == 1),
+   out[m, 64h .. 64h+63] = softmax_j(q_m . key_j / 8) . value_j (fp32 softmax, bf16 output).
+   Self-attention over the cache: group 1, ldb = the cache's row stride, kv_index = the step-major index table.
+   Cross-attention: group = beam, Tk = h * w, ldb = Tk * ldkv over K|V projected once per image. */
+int vtx_attn_decode(const void* q, int64_t ldq, const void* k, const void* v, int64_t ldkv, int64_t ldb,
+                    const int32_t* kv_index, int64_t ld_index, void* out, int64_t ldo, int blocks, int heads, int group,
+                    int Tk, void* stream);
+/* Row half of a beam step, one row of fp32 logits [R, ldl] (V columns, bias included) per CTA: scores = log_softmax
+   in fp32, then exactly -10000 at the row's last token last[row], then -- when last[row] == eos -- 0 at eos and -inf
+   elsewhere, unnormalised (beam_search.py:152-172).  last == NULL: log_softmax only (the first step).  Writes the k
+   best scores and their columns, cand_val fp32 / cand_idx int32 [R, k], in descending order, equal scores in ascending
+   column order (as vtx_topk_rows); NaN ranks as -inf.  k <= min(V, 32). */
+int vtx_beam_rows(const float* logits, int64_t ldl, int R, int V, const int64_t* last, int eos, int k, float* cand_val,
+                  int32_t* cand_idx, void* stream);
+/* Image half of a beam step, one warp per image b < B.  Candidate c < parents * k of image b is row candidate c % k of
+   parent row p = b * parents + c / k, scored cand_val + scores_in[p] (0 when scores_in is NULL).  The beam best
+   candidates (descending, ties in ascending c) become rows i = b * beam + r:
+       scores_out[i] = score,  parent_out[i] = p (optional),  pred_out[s, i] = cand_idx,  index_out[s, i] = i,
+       pred_out[j, i] = pred_in[j, p] and index_out[j, i] = index_in[j, p] for j < s,
+   and alive[s] = 1 if any new token is not eos (alive is zeroed by the caller).  scores_in may alias scores_out;
+   the tables may not alias (ping-pong them).  beam <= parents * k <= 32. */
+int vtx_beam_select(const float* cand_val, const int32_t* cand_idx, int parents, int k, int beam, const float* scores_in,
+                    float* scores_out, int32_t* parent_out, const int64_t* pred_in, int64_t* pred_out,
+                    const int32_t* index_in, int32_t* index_out, int B, int s, int eos, int32_t* alive, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * GPU input pipeline (csrc/input_pipe.cu): decoded uint8 HWC images -> fp32 NCHW network input, token lists -> padded
  * matrices.  Replaces the per-sample albumentations / cv2 transforms and the collate of
  * virtex/data/datasets/captioning.py:51-100 with the transform lists of virtex/factories.py:131-155.  Random parameters

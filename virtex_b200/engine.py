@@ -29,6 +29,7 @@ from .ops import call, gemm, _p, _stream
 
 BF16, F32 = torch.bfloat16, torch.float32
 _ALIGN = 64  # arena alignment in elements (256 B for fp32, 128 B for bf16: TMA base pointers need 16 B)
+DECODE_MAX_KEYS = 64  # VTX_DECODE_MAX_KEYS of include/virtex_b200.h
 
 
 def _round_up(x, m):
@@ -739,23 +740,13 @@ class Engine:
             lr = dict(q=f"{d}.transformer.layers.{l}.", k=k, sb=site + 10 * (l + 1))
             pr = ws.get(k + "proj", (M, H), BF16)
             for i, sublayer in enumerate((self._self_attn_fwd, self._cross_attn_fwd, self._ffn_fwd), 1):
-                norm = f"{lr['q']}norm{i}."
-                w, b = self.P(norm + "weight").data_ptr(), self.P(norm + "bias").data_ptr()
                 z, st = ws.get(f"{k}z{i}", (M, H), F32), ws.get(f"{k}st{i}", (M, 2), F32)
                 xo = ws.get(f"{k}x{i}", (M, H), F32)
+                xb_out = ws.get(f"{k}n{i}b" if mod.norm_first else f"{k}x{i}b", (M, H), BF16)
                 site_i = lr["sb"] + 2 * i - 1  # the branch's dropout before the residual add
-                if mod.norm_first:  # x + dropout(f(LN(x))) (torch/nn/modules/transformer.py:1131-1143)
-                    xb = ws.get(f"{k}n{i}b", (M, H), BF16)
-                    call("vtx_add_ln_fwd", x.data_ptr(), 0, w, b, z.data_ptr(), st.data_ptr(), 0, xb.data_ptr(), M, H,
-                         1e-5, 0.0, seed, 0, 1, s)
-                    sublayer(rec, lr, xb, pr)
-                    call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), 0, 0, xo.data_ptr(), 0, 0, 0, M, H, 0.0, p,
-                         seed, site_i, 0, s)
-                else:  # LN(x + dropout(f(x))), with a bf16 shadow of the result for the next sublayer's GEMMs
-                    sublayer(rec, lr, xb, pr)
-                    xb = ws.get(f"{k}x{i}b", (M, H), BF16)
-                    call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), w, b, z.data_ptr(), st.data_ptr(),
-                         xo.data_ptr(), xb.data_ptr(), M, H, 1e-5, p, seed, site_i, 1, s)
+                xb = self._residual_sublayer(mod.norm_first, f"{lr['q']}norm{i}.",
+                                             lambda inp, out: sublayer(rec, lr, inp, out), x, xb, xo, xb_out, pr, z, st,
+                                             M, H, p, site_i)
                 x = xo
                 lr.update({f"z{i}": z, f"st{i}": st})
             rec["layers"].append(lr)
@@ -778,6 +769,25 @@ class Engine:
         gemm(xb, wv, logits, M, V, H, bias=bo)
         rec["logits"] = logits
         return rec
+
+    def _residual_sublayer(self, norm_first, norm, run, x, xb, xo, xb_out, pr, z, st, M, H, p, site):
+        """One residual sublayer of a decoder layer, fp32 residual stream x [M, H] (bf16 shadow xb) -> xo, where
+        `run(inp, pr)` writes the branch f(inp) of the bf16 input to pr and `norm` names the sublayer's LayerNorm.
+        Pre-norm: xo = x + dropout(f(LN(x))), LN(x) in xb_out.  Post-norm: xo = LN(x + dropout(f(x))), its bf16 shadow
+        in xb_out (the next sublayer's input).  z / st receive the LayerNorm's input and statistics; returns xb_out."""
+        s, seed = _stream(), self.seed.data_ptr()
+        w, b = self.P(norm + "weight").data_ptr(), self.P(norm + "bias").data_ptr()
+        if norm_first:  # torch/nn/modules/transformer.py:1131-1143
+            call("vtx_add_ln_fwd", x.data_ptr(), 0, w, b, z.data_ptr(), st.data_ptr(), 0, xb_out.data_ptr(), M, H, 1e-5,
+                 0.0, seed, 0, 1, s)
+            run(xb_out, pr)
+            call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), 0, 0, xo.data_ptr(), 0, 0, 0, M, H, 0.0, p, seed, site, 0,
+                 s)
+        else:
+            run(xb, pr)
+            call("vtx_add_ln_fwd", x.data_ptr(), pr.data_ptr(), w, b, z.data_ptr(), st.data_ptr(), xo.data_ptr(),
+                 xb_out.data_ptr(), M, H, 1e-5, p, seed, site, 1, s)
+        return xb_out
 
     def _attn_fwd(self, rec, q, k, v, o, lse, Tk, lengths, mask_mode, site):
         """Multi-head attention of the T query rows of each caption over its Tk key rows.  q, k, v, o: row-major views
@@ -1074,6 +1084,166 @@ class Engine:
         out = self.ws.get("pred", (rec["M"],), torch.int64)
         call("vtx_argmax_rows", lf.data_ptr(), lf.stride(0), rec["M"], lf.shape[1], out.data_ptr(), _stream())
         return out.view(rec["B"], rec["T"])
+
+    # ------------------------------------------------------------------------------------------------ beam search
+    # AutoRegressiveBeamSearch (virtex/utils/beam_search.py:52-238) over CaptioningModel.decoding_step
+    # (virtex/models/captioning.py:144-213), eval mode, forward-direction head only.  The reference recomputes the whole
+    # prefix every step; here each step runs the decoder on one new position per beam row:
+    #   * step 0 decodes [SOS] once per image (B rows, position 0, a one-slot self-attention cache of its own);
+    #   * step t >= 1 decodes the beam's token t-1 at position t-1 (the reference's input drops SOS, so step 0's state
+    #     is not a prefix of step 1's); its self-attention K|V go straight from the in-projection GEMM into slot t-1 of
+    #     the row's cache, and attention reads slots 0..t-1 through the step-major index table, in which the beam
+    #     selection gathers each surviving beam's ancestry -- the caches themselves are never moved;
+    #   * cross-attention K|V of the image features are projected once per image and layer, shared by its beams.
+    # Every buffer is a workspace key of the search's own ("bs."): a pending backward's tape is left alone.
+    def beam_search(self, image, beam_size, per_node, max_steps, sos, eos):
+        """image fp32 NCHW [B,3,H,W] -> int64 (B, L) on the device: the best beam of each image, EOS repeated after
+        its first EOS; L <= max_steps is the number of steps run before every beam of every image ended in EOS."""
+        st = self.beam_start(image, beam_size, per_node, max_steps, sos, eos)
+        while st.L < max_steps and st.alive[st.L - 1].item():  # one device-to-host read per step
+            self.beam_step(st)
+        return st.best()
+
+    def beam_start(self, image, beam_size, per_node, max_steps, sos, eos):
+        """Backbone (folded BN), visual projection, cross-attention K|V of every layer, and step 0 -> the search
+        state (_BeamState) after its first step."""
+        mod = self.textual
+        if max_steps - 1 > mod.max_caption_length:
+            raise ValueError(f"max_steps {max_steps} needs {max_steps - 1} positions; the head has "
+                             f"{mod.max_caption_length}")
+        # vtx_attn_decode attends over at most DECODE_MAX_KEYS keys: the max_steps - 1 cache slots of self-attention
+        # and the h * w feature positions of cross-attention (h = w = 8 for a 256 x 256 image)
+        h, w = image.shape[2], image.shape[3]
+        for _ in range(5):  # stem conv, max-pool, layer2..4: each (x - 1) // 2 + 1
+            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        if max_steps - 1 > DECODE_MAX_KEYS or h * w > DECODE_MAX_KEYS:
+            raise ValueError(f"beam search attends over at most {DECODE_MAX_KEYS} keys: max_steps {max_steps} needs "
+                             f"{max_steps - 1}, a {image.shape[2]} x {image.shape[3]} image {h * w} feature positions")
+        self.mark_weights_dirty()  # parameters may have been updated by any optimiser since the last call
+        feat, h, w = self.backbone_infer(image)
+        B, Sk, ws = image.shape[0], h * w, self.ws
+        H, V, R = mod.hidden_size, mod.vocab_size, B * beam_size
+        mem = ws.get("bs.mem", (B * Sk, H), BF16)
+        gemm(feat, self.W("textual.visual_projection.weight"), mem, B * Sk, H, feat.shape[1],
+             bias=self.P("textual.visual_projection.bias"))
+        ckv = []
+        for l in range(mod.num_layers):
+            q = f"textual.transformer.layers.{l}.multihead_attn."
+            kv = ws.get(f"bs.ckv{l}", (B * Sk, 2 * H), BF16)
+            gemm(mem, self.W(q + "in_proj_weight")[H:], kv, B * Sk, 2 * H, H, bias=self.P(q + "in_proj_bias")[H:])
+            ckv.append(kv)
+        st = _BeamState(B=B, beam=beam_size, per_node=per_node, max_steps=max_steps, eos=eos, R=R, Sk=Sk, ckv=ckv, L=1,
+                        cur=0)
+        st.cache = [ws.get(f"bs.cache{l}", (R, max_steps - 1, 2 * H), BF16) for l in range(mod.num_layers)]
+        st.cache0 = [ws.get(f"bs.cache0.{l}", (B, 1, 2 * H), BF16) for l in range(mod.num_layers)]
+        st.pred = [ws.get(f"bs.pred{i}", (max_steps, R), torch.int64) for i in (0, 1)]
+        st.index = [ws.get(f"bs.index{i}", (max_steps, R), torch.int32) for i in (0, 1)]
+        st.scores = ws.get("bs.scores", (R,), F32)
+        st.parent = ws.get("bs.parent", (R,), torch.int32)
+        st.alive = ws.get("bs.alive", (max_steps,), torch.int32)
+        st.alive.zero_()
+        st.logits = ws.get("bs.logits", (R, V), F32)
+        sos_t = ws.get("bs.sos", (B,), torch.int64)
+        sos_t.fill_(sos)
+        self._decode_position(st, B, sos_t, 0, 1, st.cache0, None)
+        self._beam_select(st, B, None, beam_size, 1, 0)
+        return st
+
+    def beam_step(self, st):
+        """Step t = st.L: decode token t-1 of every beam at position t-1, score, select; st.L becomes t + 1."""
+        t, R, cur = st.L, st.R, st.cur
+        tokens = st.pred[cur][t - 1]
+        self._decode_position(st, R, tokens, t - 1, st.beam, st.cache, st.index[cur])
+        self._beam_select(st, R, tokens, st.per_node, st.beam, t)
+        st.cur, st.L = 1 - cur, t + 1
+
+    def _beam_select(self, st, rows, last, k, parents, s):
+        """Both halves of a beam step over st.logits [rows, V]: per-row top-k, then per-image selection into the other
+        ping-pong tables (step 0 writes table 0 directly)."""
+        V = self.textual.vocab_size
+        cv = self.ws.get("bs.cand_val", (rows, k), F32)
+        ci = self.ws.get("bs.cand_idx", (rows, k), torch.int32)
+        call("vtx_beam_rows", st.logits.data_ptr(), V, rows, V, _p(last), st.eos, k, cv.data_ptr(), ci.data_ptr(),
+             _stream())
+        src, dst = (st.cur, 1 - st.cur) if s > 0 else (None, 0)
+        call("vtx_beam_select", cv.data_ptr(), ci.data_ptr(), parents, k, st.beam, st.scores.data_ptr() if s > 0 else 0,
+             st.scores.data_ptr(), st.parent.data_ptr(), 0 if src is None else st.pred[src].data_ptr(),
+             st.pred[dst].data_ptr(), 0 if src is None else st.index[src].data_ptr(), st.index[dst].data_ptr(), st.B, s,
+             st.eos, st.alive.data_ptr(), _stream())
+
+    def _decode_position(self, st, rows, tokens, pos, group, cache, index):
+        """Forward head on one new position: tokens int64 [rows] at position `pos`, self-attention over cache slots
+        0..pos (slot pos written here; through `index` when given), cross-attention of row m over image m // group
+        -> fp32 logits st.logits[:rows]."""
+        mod = self.textual
+        H, A, Fd, V = mod.hidden_size, mod.attention_heads, mod.feedforward_size, mod.vocab_size
+        ws, s, seed = self.ws, _stream(), self.seed.data_ptr()
+        emb = "textual.embedding."
+        xs = [ws.get(f"bs.x{i}", (rows, H), F32) for i in (0, 1)]
+        z, zst = ws.get("bs.z", (rows, H), F32), ws.get("bs.st", (rows, 2), F32)
+        xb = ws.get("bs.xb", (rows, H), BF16)
+        # the embedding kernel with T = 1 over position row `pos` is the one-position embedding
+        call("vtx_embed_fwd", tokens.data_ptr(), self.P(emb + "words.weight").data_ptr(),
+             self.P(emb + "positions.weight")[pos].data_ptr(), self.P(emb + "layer_norm.weight").data_ptr(),
+             self.P(emb + "layer_norm.bias").data_ptr(), z.data_ptr(), zst.data_ptr(), xs[0].data_ptr(), xb.data_ptr(),
+             rows, 1, H, self.pad, 1e-8, 0.0, seed, 0, s)
+        qb, o = ws.get("bs.q", (rows, H), BF16), ws.get("bs.o", (rows, H), BF16)
+        pr = ws.get("bs.proj", (rows, H), BF16)
+        xbs = [ws.get(f"bs.xb{i}", (rows, H), BF16) for i in (0, 1)]
+        n = 0
+        for l in range(mod.num_layers):
+            q = f"textual.transformer.layers.{l}."
+            c = cache[l]
+
+            def self_attn(inp, out):
+                w, b = self.W(q + "self_attn.in_proj_weight"), self.P(q + "self_attn.in_proj_bias")
+                gemm(inp, w[:H], qb, rows, H, H, bias=b[:H])
+                gemm(inp, w[H:], c, rows, 2 * H, H, bias=b[H:], ldd=c.stride(0),
+                     d_ptr=c.data_ptr() + pos * c.stride(1) * c.element_size())
+                call("vtx_attn_decode", qb.data_ptr(), H, c.data_ptr(), c.data_ptr() + H * c.element_size(), c.stride(1),
+                     c.stride(0), _p(index), rows, o.data_ptr(), H, rows, A, 1, pos + 1, s)
+                gemm(o, self.W(q + "self_attn.out_proj.weight"), out, rows, H, H, bias=self.P(q + "self_attn.out_proj.bias"))
+
+            def cross_attn(inp, out):
+                w, b = self.W(q + "multihead_attn.in_proj_weight"), self.P(q + "multihead_attn.in_proj_bias")
+                gemm(inp, w[:H], qb, rows, H, H, bias=b[:H])
+                kv = st.ckv[l]
+                call("vtx_attn_decode", qb.data_ptr(), H, kv.data_ptr(), kv.data_ptr() + H * kv.element_size(), 2 * H,
+                     st.Sk * 2 * H, 0, 0, o.data_ptr(), H, rows // group, A, group, st.Sk, s)
+                gemm(o, self.W(q + "multihead_attn.out_proj.weight"), out, rows, H, H,
+                     bias=self.P(q + "multihead_attn.out_proj.bias"))
+
+            def ffn(inp, out):
+                self._ffn_fwd(dict(M=rows, H=H, Fd=Fd, p=0.0), dict(q=q, k="bs.", sb=0), inp, out)
+
+            for i, run in enumerate((self_attn, cross_attn, ffn), 1):
+                xb = self._residual_sublayer(mod.norm_first, f"{q}norm{i}.", run, xs[n & 1], xb, xs[1 - (n & 1)],
+                                             xbs[n & 1], pr, z, zst, rows, H, 0.0, 0)
+                n += 1
+        if mod.norm_first:  # final LayerNorm of pre-norm decoders
+            qn = "textual.transformer.norm."
+            xb = xbs[n & 1]
+            call("vtx_add_ln_fwd", xs[n & 1].data_ptr(), 0, self.P(qn + "weight").data_ptr(),
+                 self.P(qn + "bias").data_ptr(), z.data_ptr(), zst.data_ptr(), 0, xb.data_ptr(), rows, H, 1e-5, 0.0, seed,
+                 0, 1, s)
+        gemm(xb, self.W("textual.embedding.words.weight"), st.logits, rows, V, H, bias=self.P("textual.output.bias"))
+
+
+class _BeamState:
+    """Buffers and progress of one running beam search (Engine.beam_start / beam_step): L steps have run; the current
+    step-major tables are pred[cur] (int64 [max_steps, B * beam]) and index[cur]; scores holds each beam's sum of
+    log-probabilities, st.logits the fp32 logits of the last step."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def tokens(self):
+        """int64 (B * beam, L): every beam's tokens so far."""
+        return self.pred[self.cur][:self.L].t()
+
+    def best(self):
+        """int64 (B, L): beam 0 of every image (the best, beams are kept in descending score order)."""
+        return self.tokens()[::self.beam].contiguous()
 
 
 # ---------------------------------------------------------------------------------------------------- module-level API

@@ -82,19 +82,22 @@ class TextualHeadFactory(Factory):
 
 
 class _DecoderSpec:
-    """Inert stand-in for the reference's beam-search / nucleus-sampling objects: the captioning model only *stores* its
-    decoder during pretraining (virtex/models/captioning.py:68); autoregressive decoding is outside the hot path."""
+    """Parameters of the reference's beam-search / nucleus-sampling objects.  A captioning model with a `beam_search`
+    decoder captions images by the engine's incremental beam search (CaptioningModel.forward without caption_tokens),
+    which reads its parameters from here; the search itself does not run on this object.  `beam_search` takes the
+    reference's per-node beam size of 2, which its factory never overrides (virtex/utils/beam_search.py:40-50,
+    virtex/factories.py:491-500).  Nucleus sampling is not implemented."""
 
     def __init__(self, name, **kwargs):
         self.name = name
         self.__dict__.update(kwargs)
 
     def search(self, *a, **k):
-        raise NotImplementedError("autoregressive decoding is outside the bicaptioning pretraining hot path")
+        raise NotImplementedError("decoding runs inside CaptioningModel.forward on the engine")
 
 
 class CaptionDecoderFactory(Factory):
-    PRODUCTS: Dict[str, Callable] = {"beam_search": partial(_DecoderSpec, "beam_search"),
+    PRODUCTS: Dict[str, Callable] = {"beam_search": partial(_DecoderSpec, "beam_search", per_node_beam_size=2),
                                      "nucleus_sampling": partial(_DecoderSpec, "nucleus_sampling")}
 
     @classmethod

@@ -117,7 +117,7 @@ class CaptioningModel(_EngineModel):
         if "caption_tokens" not in batch:
             if self.decoder is None:
                 raise ValueError("Decoder for predicting captions is missing!")
-            raise NotImplementedError("autoregressive decoding is outside the bicaptioning pretraining hot path")
+            return {"predictions": self._beam_search(batch["image"])}
         image = batch["image"]
         if image.device.type != "cuda":
             raise RuntimeError("virtex_b200 has no CPU path: the batch must live on the model's CUDA device")
@@ -140,8 +140,31 @@ class CaptioningModel(_EngineModel):
             output["predictions"] = eng.predictions().clone()
         return output
 
+    def _beam_search(self, image):
+        """Captions of the forward-direction head by the reference's beam search (captioning.py:144-163), decoded
+        incrementally by the engine: int64 (B, L) on the device."""
+        dec = self.decoder
+        if dec.name != "beam_search":
+            raise NotImplementedError(f"{dec.name} decoding is not implemented; beam_search is")
+        if self.training:
+            raise RuntimeError("beam search runs in eval mode (running BatchNorm statistics, no dropout): call "
+                               "model.eval() first")
+        if image.device.type != "cuda":
+            raise RuntimeError("virtex_b200 has no CPU path: the batch must live on the model's CUDA device")
+        with torch.no_grad():
+            return self.engine.beam_search(image.contiguous().float(), dec.beam_size, dec.per_node_beam_size,
+                                           dec.max_steps, self.sos_index, dec.eos_index)
+
     def decoding_step(self, visual_features, partial_captions):
-        raise NotImplementedError("autoregressive decoding is outside the bicaptioning pretraining hot path")
+        """Logits of the next token of every partial caption (captioning.py:165-213): (B, C, h, w) fp32 features and
+        (B * beam, T) tokens, or (B * beam,) for the first step -> fp32 (B * beam, V).  The whole prefix is recomputed by
+        the textual head; the reference's own decoders can drive this model through it."""
+        tokens = partial_captions if partial_captions.dim() == 2 else partial_captions[:, None]
+        rows, prefix = tokens.shape
+        per_image = rows // visual_features.shape[0]  # the beams of image b are rows b * per_image ...
+        features = visual_features.repeat_interleave(per_image, 0) if per_image > 1 else visual_features
+        lengths = torch.full((rows,), prefix, dtype=torch.int64, device=tokens.device)  # no padding in a prefix
+        return self.textual(features, tokens, lengths)[:, -1]
 
 
 class ForwardCaptioningModel(CaptioningModel):

@@ -54,6 +54,9 @@ _PROTOS = {
     "vtx_group_mean_bwd": [P, P, I, I, I, P],
     "vtx_khot_xent": [P, I64, P, I64, I, I, I, P, I, P, I, P],
     "vtx_topk_rows": [P, I64, I, I, I, P, P],
+    "vtx_attn_decode": [P, I64, P, P, I64, I64, P, I64, P, I64, I, I, I, I, P],
+    "vtx_beam_rows": [P, I64, I, I, P, I, I, P, P, P],
+    "vtx_beam_select": [P, P, I, I, I, P, P, P, P, P, P, P, I, I, I, P, P],
     "vtx_image_resample": [P, P, P, P, P, P, I, I, P],
     "vtx_image_gray_sum": [P, P, P, P, I, I, P],
     "vtx_image_jitter_normalize": [P, P, P, P, P, P, I, I, P],
