@@ -328,6 +328,11 @@ int vtx_sumsq(const float* x, int64_t n, float* out, void* stream);
 int vtx_clip_coef(const float* sumsq, int world_size, float max_norm, float* ctl, void* stream);
 int vtx_sgd_step(float* p, const float* g, float* mom, float* slow, void* p_bf, const void* segs, int nseg,
                  const float* ctl, const float* hyper, float momentum, float la_alpha, void* stream);
+/* torch.optim.AdamW (decoupled weight decay, no amsgrad) over the same segments; elements outside every segment and
+ * their moments are left untouched.  hyper = {lr multiplier, 1/(1-beta1^t), 1/sqrt(1-beta2^t), lookahead}. */
+int vtx_adamw_step(float* p, const float* g, float* exp_avg, float* exp_avg_sq, float* slow, void* p_bf,
+                   const void* segs, int nseg, const float* ctl, const float* hyper, double beta1, double beta2,
+                   float eps, float la_alpha, void* stream);
 
 #ifdef __cplusplus
 }

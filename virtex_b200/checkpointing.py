@@ -6,9 +6,12 @@ written by either implementation loads into the other:
 
   * the model's `state_dict` has the reference's 370 keys (tests/test_host_cpu.py);
   * `FusedOptimizerState` / `FusedSchedulerState` present the fused device-side optimiser tail of
-    `virtex_b200.trainer.Trainer` (flat momentum arena, per-name lr / weight decay, step counter) in the
-    `torch.optim.SGD` / `LambdaLR` state-dict layouts the reference's `Lookahead(SGD)` + `LinearWarmup*LR` serialise:
-    one param group per parameter in `named_parameters()` order, `momentum_buffer` per parameter index, `last_epoch`.
+    `virtex_b200.trainer.Trainer` (flat moment arenas, per-name lr / weight decay, step counter) in the state-dict
+    layouts the reference's `Lookahead(SGD)` or `Lookahead(AdamW)` + `LinearWarmup*LR` serialise, chosen by
+    OPTIM.OPTIMIZER_NAME: one param group per parameter in `named_parameters()` order, `last_epoch`, and per trainable
+    parameter index either `momentum_buffer` (torch.optim.SGD) or `step` / `exp_avg` / `exp_avg_sq`
+    (torch.optim.AdamW; `step` a 0-dim float32 tensor, the same for every parameter since the fused tail keeps one
+    step count -- a file whose parameters disagree on it is refused).  The state is empty before the first step.
     As in the reference, Lookahead's slow weights and k-counter are not part of the state (lookahead.py:61-66): after
     a load the slow weights restart from the loaded parameters.
 """
@@ -21,6 +24,7 @@ from torch import nn
 
 from . import distributed as vdist
 from .factories import param_group_hparams
+from .trainer import ADAMW_BETAS, ADAMW_EPS
 
 
 def _unwrap(obj):
@@ -77,13 +81,17 @@ class CheckpointManager:
 # ------------------------------------------------------------------------------------- fused optimiser tail <-> torch
 _SGD_DEFAULTS = {"dampening": 0, "nesterov": False, "maximize": False, "foreach": None, "differentiable": False,
                  "fused": None}
+_ADAMW_DEFAULTS = {"betas": ADAMW_BETAS, "eps": ADAMW_EPS, "amsgrad": False, "maximize": False, "foreach": None,
+                   "capturable": False, "differentiable": False, "fused": None, "decoupled_weight_decay": True}
 
 
 class FusedOptimizerState:
-    """`torch.optim.SGD`-layout view of a Trainer's momentum arena (one param group per parameter, by name)."""
+    """`torch.optim.SGD`- or `torch.optim.AdamW`-layout view of a Trainer's moment arenas (one param group per
+    parameter, by name), after OPTIM.OPTIMIZER_NAME."""
 
     def __init__(self, trainer):
         self._t = trainer
+        self._adamw = trainer.config.OPTIM.OPTIMIZER_NAME == "adamw"
 
     def _hparams(self):
         t = self._t
@@ -95,14 +103,20 @@ class FusedOptimizerState:
         mult = t.lr_fn(t.iteration)
         groups = []
         for i, (lr, wd) in enumerate(self._hparams()):
-            g = {"lr": lr * mult, "weight_decay": wd, "momentum": t.momentum}
-            g.update(_SGD_DEFAULTS)
+            if self._adamw:
+                g = {"lr": lr * mult, "weight_decay": wd}
+                g.update(_ADAMW_DEFAULTS)
+            else:
+                g = {"lr": lr * mult, "weight_decay": wd, "momentum": t.momentum}
+                g.update(_SGD_DEFAULTS)
             g["initial_lr"] = lr
             g["params"] = [i]
             groups.append(g)
         return groups
 
     def state_dict(self) -> Dict[str, Any]:
+        if self._adamw:
+            return self._adamw_state_dict()
         t = self._t
         a = t.arena
         state = {}
@@ -112,13 +126,19 @@ class FusedOptimizerState:
                     state[i] = {"momentum_buffer": a.view(t.mom, n).detach().clone()}
         return {"state": state, "param_groups": self.param_groups}
 
+    def _check_groups(self, groups):
+        n = len(self._t.arena.names)
+        if len(groups) != n or any(len(g["params"]) != 1 for g in groups):
+            raise ValueError(f"expected one parameter group per parameter ({n} groups, as built by "
+                             f"OptimizerFactory.from_config); the checkpoint has {len(groups)}")
+
     def load_state_dict(self, state_dict: Dict[str, Any]):
+        if self._adamw:
+            return self._adamw_load_state_dict(state_dict)
         t = self._t
         a = t.arena
         groups = state_dict["param_groups"]
-        if len(groups) != len(a.names) or any(len(g["params"]) != 1 for g in groups):
-            raise ValueError(f"expected one parameter group per parameter ({len(a.names)} groups, as built by "
-                             f"OptimizerFactory.from_config); the checkpoint has {len(groups)}")
+        self._check_groups(groups)
         state = state_dict.get("state", {})
         t.mom.zero_()
         ready = False
@@ -133,6 +153,57 @@ class FusedOptimizerState:
                 a.view(t.mom, n).copy_(buf.to(device=t.mom.device, dtype=t.mom.dtype))
                 ready = True
         t.momentum_ready = ready
+        t.reset_lookahead()
+
+    # ---------------------------------------------------------------------------------------------------- AdamW
+    def _adamw_state_dict(self) -> Dict[str, Any]:
+        t = self._t
+        a = t.arena
+        state = {}
+        if t.adam_step >= 1:
+            for i, n in enumerate(a.names):
+                if a._param_objs[n].requires_grad:
+                    state[i] = {"step": torch.tensor(float(t.adam_step), dtype=torch.float32),
+                                "exp_avg": a.view(t.exp_avg, n).detach().clone(),
+                                "exp_avg_sq": a.view(t.exp_avg_sq, n).detach().clone()}
+        return {"state": state, "param_groups": self.param_groups}
+
+    def _adamw_load_state_dict(self, state_dict: Dict[str, Any]):
+        t = self._t
+        a = t.arena
+        groups = state_dict["param_groups"]
+        state = state_dict.get("state", {})
+        if any("momentum_buffer" in st for st in state.values()) or any("betas" not in g for g in groups):
+            raise ValueError("the checkpoint holds a torch.optim.SGD state; this Trainer runs AdamW "
+                             "(OPTIM.OPTIMIZER_NAME adamw)")
+        self._check_groups(groups)
+        for g in groups:
+            if (tuple(g["betas"]) != ADAMW_BETAS or g["eps"] != ADAMW_EPS or g.get("amsgrad", False)
+                    or g.get("maximize", False)):
+                raise ValueError(f"the fused AdamW runs betas {ADAMW_BETAS}, eps {ADAMW_EPS}, no amsgrad / maximize; "
+                                 f"the checkpoint has betas {g['betas']}, eps {g['eps']}, amsgrad {g.get('amsgrad')}, "
+                                 f"maximize {g.get('maximize')}")
+        entries, steps = [], set()
+        for n, g in zip(a.names, groups):
+            if not a._param_objs[n].requires_grad:
+                continue
+            st = state.get(g["params"][0], state.get(str(g["params"][0])))
+            steps.add(0 if st is None else int(round(float(st["step"]))))
+            if st is not None:
+                for k in ("exp_avg", "exp_avg_sq"):
+                    if tuple(st[k].shape) != tuple(a.shapes[n]):
+                        raise ValueError(f"{k} of {n}: shape {tuple(st[k].shape)} != {tuple(a.shapes[n])}")
+                entries.append((n, st))
+        if len(steps) > 1:
+            raise ValueError(f"the trainable parameters of the checkpoint have different AdamW step counts "
+                             f"{sorted(steps)}; the fused optimiser tail keeps one step count for all of them")
+        t.exp_avg.zero_()
+        t.exp_avg_sq.zero_()
+        with torch.no_grad():
+            for n, st in entries:
+                a.view(t.exp_avg, n).copy_(st["exp_avg"].to(device=t.exp_avg.device, dtype=t.exp_avg.dtype))
+                a.view(t.exp_avg_sq, n).copy_(st["exp_avg_sq"].to(device=t.exp_avg_sq.device, dtype=t.exp_avg_sq.dtype))
+        t.adam_step = steps.pop() if steps else 0
         t.reset_lookahead()
 
 

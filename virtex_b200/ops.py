@@ -4,13 +4,13 @@ Every function launches on torch's current CUDA stream, never allocates and neve
 fallback: a missing library or a non-CUDA tensor raises.
 """
 import ctypes
-from ctypes import c_float, c_int, c_int32, c_int64, c_uint32, c_void_p
+from ctypes import c_double, c_float, c_int, c_int32, c_int64, c_uint32, c_void_p
 
 import torch
 
 from . import lib as L
 
-P, I, I64, F, U32 = c_void_p, c_int, c_int64, c_float, c_uint32
+P, I, I64, F, D, U32 = c_void_p, c_int, c_int64, c_float, c_double, c_uint32
 
 _PROTOS = {
     "vtx_gemm": [P, P],
@@ -64,6 +64,7 @@ _PROTOS = {
     "vtx_sumsq": [P, I64, P, P],
     "vtx_clip_coef": [P, I, F, P, P],
     "vtx_sgd_step": [P, P, P, P, P, P, I, P, P, F, F, P],
+    "vtx_adamw_step": [P, P, P, P, P, P, P, I, P, P, D, D, F, F, P],
 }
 
 _fn = {}

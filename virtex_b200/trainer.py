@@ -1,15 +1,20 @@
 """`Trainer.step(batch)`: the reference loop body (scripts/pretrain_virtex.py:145-163) on the H100 engine.
 
     zero_grad -> forward (bf16 compute) -> backward -> [data-parallel gradient all-reduce, overlapped with backward]
-    -> global-norm clip -> SGD(momentum, per-parameter lr / weight decay) -> Lookahead every k steps -> LR schedule
+    -> global-norm clip -> SGD(momentum) or AdamW, with per-parameter lr / weight decay -> Lookahead every k steps
+    -> LR schedule
 
 The optimiser tail runs as fused kernels over the flat arenas (virtex_b200/csrc/optim.cu) with the arithmetic of
-torch.optim.SGD + virtex/optim/lookahead.py + virtex/optim/lr_scheduler.py; bf16 needs no GradScaler.
+torch.optim.SGD or torch.optim.AdamW (OPTIM.OPTIMIZER_NAME "sgd" / "adamw"; AdamW with torch's default betas and eps,
+as the reference) + virtex/optim/lookahead.py + virtex/optim/lr_scheduler.py; bf16 needs no GradScaler.  SGD keeps a
+momentum arena; AdamW keeps exp_avg / exp_avg_sq arenas and one host-side step count t, from which the host computes
+the bias corrections in double precision for each step.
 Gradient all-reduce: NCCL over NVLink on a side stream, one bucket per completed gradient range in backward order
 (backward-direction decoder; forward-direction decoder + shared embedding / projection; layer4; layer3; layer2; the
 rest), SUM on the wire and the 1/world_size folded into the clip coefficient,
 so averaged gradients equal the mean of per-rank gradients like DistributedDataParallel's.
 """
+import math
 import struct
 from typing import Dict, Optional
 
@@ -23,6 +28,8 @@ from .ops import _stream, call
 from .optim import lr_multiplier_fn
 
 _CHUNK = 65536
+OPTIMIZERS = ("sgd", "adamw")
+ADAMW_BETAS, ADAMW_EPS = (0.9, 0.999), 1e-8  # torch.optim.AdamW defaults, which the reference keeps
 # completion order of gradient ranges in backward: the backward-direction decoder finishes first (its gradients are the
 # last contiguous range of the arena), then everything shared / forward-direction of the head, then the backbone layers
 BUCKET_ORDER = ("head_b", "head", "layer4", "layer3", "layer2", "rest")
@@ -60,8 +67,9 @@ def optimizer_segments(names, offsets, numels, hparams, chunk=_CHUNK):
 
 class Trainer:
     def __init__(self, model, config: Config, process_group=None):
-        if config.OPTIM.OPTIMIZER_NAME != "sgd":
-            raise NotImplementedError("the fused optimiser tail implements the reference's SGD recipe")
+        if config.OPTIM.OPTIMIZER_NAME not in OPTIMIZERS:
+            raise NotImplementedError(f"the fused optimiser tail implements {' and '.join(OPTIMIZERS)}, "
+                                      f"not {config.OPTIM.OPTIMIZER_NAME!r}")
         self.model = model
         self.config = config
         self.engine = eng = model.engine
@@ -71,6 +79,7 @@ class Trainer:
         self.group = process_group
         O = config.OPTIM
         self.max_norm = float(O.CLIP_GRAD_NORM)
+        self.optimizer_name = O.OPTIMIZER_NAME
         self.momentum = float(O.SGD_MOMENTUM)
         self.use_lookahead = bool(O.LOOKAHEAD.USE)
         self.la_alpha = float(O.LOOKAHEAD.ALPHA)
@@ -83,7 +92,11 @@ class Trainer:
         blob = b"".join(struct.pack("<qqff", *s) for s in segs)
         self.nseg = len(segs)
         self.segs = torch.frombuffer(bytearray(blob), dtype=torch.uint8).to(dev)
-        self.mom = torch.zeros_like(arena.params)
+        if self.optimizer_name == "sgd":
+            self.mom = torch.zeros_like(arena.params)
+        else:
+            self.exp_avg = torch.zeros_like(arena.params)
+            self.exp_avg_sq = torch.zeros_like(arena.params)
         self.slow = arena.params.clone() if self.use_lookahead else None
         self.sumsq = torch.zeros(1, dtype=torch.float32, device=dev)
         self.ctl = torch.zeros(2, dtype=torch.float32, device=dev)
@@ -92,6 +105,7 @@ class Trainer:
         self.iteration = 0
         self._k_counter = 0
         self.momentum_ready = False  # torch.optim.SGD: the first step with a gradient initialises the buffer to it
+        self.adam_step = 0  # torch.optim.AdamW's step count t (one for every trainable tensor)
         # dropout seed of step i = base + i (restored from the iteration on resume); ranks get decorrelated streams
         rank = dist.get_rank(process_group) if dist.is_initialized() else 0
         self._seed_base = (int(config.RANDOM_SEED) << 24) + rank * 1000003
@@ -157,14 +171,26 @@ class Trainer:
             self._k_counter = 0
         h = self._hyper_ring[self.iteration % len(self._hyper_ring)]
         h[0] = self.lr_fn(self.iteration)  # the optimiser step of iteration i uses lambda(i - 1 + 1 - 1) = lambda(i)
-        h[1] = 0.0 if self.momentum_ready else 1.0
-        h[2] = 1.0 if do_la else 0.0
-        self.hyper.copy_(h, non_blocking=True)
-        call("vtx_sgd_step", arena.params.data_ptr(), arena.grads.data_ptr(), self.mom.data_ptr(),
-             0 if self.slow is None else self.slow.data_ptr(), arena.mirror.data_ptr(), self.segs.data_ptr(), self.nseg,
-             self.ctl.data_ptr(), self.hyper.data_ptr(), self.momentum, self.la_alpha, s)
+        slow = 0 if self.slow is None else self.slow.data_ptr()
+        if self.optimizer_name == "sgd":
+            h[1] = 0.0 if self.momentum_ready else 1.0
+            h[2] = 1.0 if do_la else 0.0
+            self.hyper.copy_(h, non_blocking=True)
+            call("vtx_sgd_step", arena.params.data_ptr(), arena.grads.data_ptr(), self.mom.data_ptr(), slow,
+                 arena.mirror.data_ptr(), self.segs.data_ptr(), self.nseg, self.ctl.data_ptr(), self.hyper.data_ptr(),
+                 self.momentum, self.la_alpha, s)
+            self.momentum_ready = True
+        else:
+            self.adam_step += 1
+            b1, b2 = ADAMW_BETAS
+            h[1] = 1.0 / (1.0 - b1 ** self.adam_step)  # bias corrections in double, as torch does with a CPU step
+            h[2] = 1.0 / math.sqrt(1.0 - b2 ** self.adam_step)
+            h[3] = 1.0 if do_la else 0.0
+            self.hyper.copy_(h, non_blocking=True)
+            call("vtx_adamw_step", arena.params.data_ptr(), arena.grads.data_ptr(), self.exp_avg.data_ptr(),
+                 self.exp_avg_sq.data_ptr(), slow, arena.mirror.data_ptr(), self.segs.data_ptr(), self.nseg,
+                 self.ctl.data_ptr(), self.hyper.data_ptr(), b1, b2, ADAMW_EPS, self.la_alpha, s)
         eng.prepare_weights(mirror=False)  # the step kernel refreshed the bf16 mirror; re-pack the k>1 conv weights
-        self.momentum_ready = True
         self.iteration += 1
 
     def sync_dropout_seed(self):
@@ -188,7 +214,8 @@ class Trainer:
 
     @property
     def optimizer(self):
-        """`torch.optim.SGD`-layout state view for checkpoint interchange (virtex_b200/checkpointing.py)."""
+        """`torch.optim.SGD`- or `torch.optim.AdamW`-layout state view for checkpoint interchange
+        (virtex_b200/checkpointing.py)."""
         from .checkpointing import FusedOptimizerState
         return FusedOptimizerState(self)
 
