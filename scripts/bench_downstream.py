@@ -1,12 +1,13 @@
 """Time the downstream classification path on one GPU (scripts/clf_linear.py, scripts/clf_voc07.py):
 
-    python scripts/bench_downstream.py [--batch 256] [--iters 20] [--warmup 5] [--rounds 3]
+    python scripts/bench_downstream.py [--arch resnet50] [--batch 256] [--iters 20] [--warmup 5] [--rounds 3]
 
-Eval-mode ResNet-50 forward at 224 x 224, three ways, alternated within one process so that clock and power drift hit
+Eval-mode forward of a torchvision ResNet (`--arch`: resnet50, resnet101, resnet152, wide_resnet50_2 or
+wide_resnet101_2) at 224 x 224, three ways, alternated within one process so that clock and power drift hit
 all three alike:
   * infer     -- Engine.backbone_infer (eval BN folded into the GEMM epilogues);
   * forward   -- Engine.backbone_forward(training=False) (raw conv outputs, then a BN + ReLU (+ residual) pass each);
-  * eager     -- torchvision ResNet-50, channels_last, bf16 autocast, cuDNN.
+  * eager     -- the same torchvision model, channels_last, bf16 autocast, cuDNN.
 Then a full linear-probe iteration (frozen eval-mode backbone, CE, SGD on fc) and a fine-tuning iteration (train mode,
 SGD on every parameter) through ResNetParams.forward.  HBM bytes of the two engine schedules are computed from the
 layer shapes (activation reads and writes of every GEMM and every elementwise pass; weights excluded), so that the
@@ -34,27 +35,29 @@ def card():
     return q
 
 
-def activation_bytes(B, H=224):
-    """(infer, forward) bytes of activations read + written by the eval forward of ResNet-50, from the shapes."""
+def activation_bytes(cnn, B, H=224):
+    """(infer, forward) bytes of activations read + written by the eval forward of `cnn` (a ResNetParams), from the
+    shapes of its weights."""
     e = 2  # bf16
     Ho = (H - 1) // 2 + 1
     Hp = (Ho - 1) // 2 + 1
     stem = B * Ho * Ho * 64 * e
     infer = fwd = stem + 2 * stem + B * Hp * Hp * 64 * e  # GEMM write, BN+ReLU+maxpool read, pool write (both)
     Hc, Cin = Hp, 64
-    for li, (planes, n) in enumerate(zip([64, 128, 256, 512], [3, 4, 6, 3]), start=1):
-        for bi in range(n):
-            stride = 2 if (bi == 0 and li > 1) else 1
+    for li in range(1, 5):
+        for blk in getattr(cnn, f"layer{li}"):
+            stride = blk.stride
+            width, C4 = blk.conv1.weight.shape[0], blk.conv3.weight.shape[0]
             Hn = (Hc - 1) // stride + 1
-            x, a1, a2, out = B * Hc * Hc * Cin * e, B * Hc * Hc * planes * e, B * Hn * Hn * planes * e, \
-                B * Hn * Hn * 4 * planes * e
-            ds = bi == 0
+            x, a1, a2, out = B * Hc * Hc * Cin * e, B * Hc * Hc * width * e, B * Hn * Hn * width * e, \
+                B * Hn * Hn * C4 * e
+            ds = blk.downsample is not None
             # folded: conv1 x -> a1, conv2 a1 -> a2, [downsample x -> shortcut], conv3 a2 + shortcut -> out
             infer += (x + a1) + (a1 + a2) + (x + out if ds else 0) + (a2 + out + out)
             # unfused: every conv writes y and a BN pass reads it back and writes the activation (+ reads the shortcut)
             fwd += (x + a1) + 2 * a1 + (a1 + a2) + 2 * a2 + (a2 + out) + (x + out if ds else 0)
             fwd += out + (out if ds else x) + out  # bn3 (+ downsample BN) + residual + ReLU pass
-            Hc, Cin = Hn, 4 * planes
+            Hc, Cin = Hn, C4
     return infer, fwd
 
 
@@ -70,6 +73,7 @@ def timed(fn, iters):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--arch", default="resnet50", help="torchvision ResNet name")
     ap.add_argument("--batch", type=int, default=256)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
@@ -80,13 +84,21 @@ def main():
         raise SystemExit("bench_downstream.py measures the GPU path: no CUDA device")
     import torchvision
     from virtex_b200.modules import ResNetParams
-    from tests import downstream_oracle as DO
+    from tests import downstream_oracle as DO, wide_oracle as WO
 
     print(f"card: {card()}", flush=True)
     torch.manual_seed(0)
     dev = torch.device("cuda")
-    state = DO.synth_state(0, a.classes)
-    cnn = ResNetParams("resnet50")
+    if a.arch == "resnet50":
+        state = DO.synth_state(0, a.classes)
+    else:  # the same recipe on the other architecture's parameter tree
+        spec = WO.spec(a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
+        state = {k[len(DO.PREFIX):]: v for k, v in WO.synth_state(spec, 0, bn3_gain=0.25).items()
+                 if k.startswith(DO.PREFIX)}
+        g = torch.Generator().manual_seed(7000)
+        state["fc.weight"] = torch.randn(a.classes, 2048, generator=g) * 0.01
+        state["fc.bias"] = torch.randn(a.classes, generator=g) * 0.1
+    cnn = ResNetParams(a.arch)
     cnn.fc = nn.Linear(2048, a.classes)
     cnn.load_state_dict(state, strict=True)
     cnn = cnn.to(dev).eval()
@@ -95,7 +107,7 @@ def main():
     with torch.no_grad():
         cnn(image[:2])  # builds the engine
     eng = cnn._vtx_engine
-    tv = torchvision.models.resnet50(num_classes=a.classes)
+    tv = getattr(torchvision.models, a.arch)(num_classes=a.classes)
     tv.load_state_dict(state, strict=True)
     tv = tv.to(dev).to(memory_format=torch.channels_last).eval()
     image_cl = image.contiguous(memory_format=torch.channels_last)
@@ -131,7 +143,7 @@ def main():
         opt.step()
 
     # fine-tuning: train mode, every parameter
-    ft = ResNetParams("resnet50")
+    ft = ResNetParams(a.arch)
     ft.fc = nn.Linear(2048, a.classes)
     ft.load_state_dict(state, strict=True)
     ft = ft.to(dev).train()
@@ -150,9 +162,10 @@ def main():
     for k, fn in iters.items():
         times[k] = [timed(fn, a.iters) for _ in range(a.rounds)]
 
-    b_inf, b_fwd = activation_bytes(a.batch)
+    b_inf, b_fwd = activation_bytes(cnn, a.batch)
     best = {k: min(v) for k, v in times.items()}
-    res = {"batch": a.batch, "image": 224, "card": card(), "ms": {k: [round(x, 3) for x in v] for k, v in times.items()},
+    res = {"arch": a.arch, "batch": a.batch, "image": 224, "card": card(),
+           "ms": {k: [round(x, 3) for x in v] for k, v in times.items()},
            "best_ms": {k: round(v, 3) for k, v in best.items()},
            "activation_bytes": {"infer": b_inf, "forward": b_fwd},
            "activation_GBps": {"infer": round(b_inf / best["infer"] / 1e6, 1),

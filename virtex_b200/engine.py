@@ -122,6 +122,12 @@ def _require_cuda(dev):
         raise RuntimeError("virtex_b200 has no CPU path: move the model to a CUDA device first (model.cuda())")
 
 
+def _block_widths(blk):
+    """(inner width of conv1 / conv2, output width of conv3) of a bottleneck, read from its weights: 4x apart for
+    ResNet-50/101/152, 2x for the wide models."""
+    return blk.conv1.weight.shape[0], blk.conv3.weight.shape[0]
+
+
 class Engine:
     """Forward/backward of (backbone) + (forward head) + (backward head) on one GPU.  Any part may be absent."""
 
@@ -285,10 +291,10 @@ class Engine:
         """(name, channels) of every BatchNorm of the backbone."""
         out = [("visual.cnn.bn1", 64)]
         for name, blk in self.blocks:
-            planes = blk.conv1.weight.shape[0]
-            out += [(name + ".bn1", planes), (name + ".bn2", planes), (name + ".bn3", 4 * planes)]
+            width, C4 = _block_widths(blk)
+            out += [(name + ".bn1", width), (name + ".bn2", width), (name + ".bn3", C4)]
             if blk.downsample is not None:
-                out.append((name + ".downsample.1", 4 * planes))
+                out.append((name + ".downsample.1", C4))
         return out
 
     def _pack_buf(self, key, shape):
@@ -323,8 +329,8 @@ class Engine:
         """One zeroed fp32 slab per step holding every BN's [2,C] sum/sumsq (fwd) and [2,C] dz sums (bwd)."""
         total = 2 * 64 * 2
         for name, blk in self.blocks:
-            planes = blk.conv1.weight.shape[0]
-            total += 2 * 2 * (planes + planes + 4 * planes + (4 * planes if blk.downsample is not None else 0))
+            width, C4 = _block_widths(blk)
+            total += 2 * 2 * (width + width + C4 + (C4 if blk.downsample is not None else 0))
         slab = self.ws.get("bn_slab", (total,), F32)
         slab.zero_()
         self._slab, self._slab_off = slab, 0
@@ -357,22 +363,22 @@ class Engine:
         return None, cols
 
     def _conv2(self, name, a1, y, B, Hc, Wc, stride, key, **epi):
-        """3x3 conv2 (stride) of block `name`: a1 [B*Hc*Wc, planes] -> y [Mout, planes]; returns the im2col matrix
+        """3x3 conv2 (stride) of block `name`: a1 [B*Hc*Wc, width] -> y [Mout, width]; returns the im2col matrix
         when that route ran, else None."""
-        Mout, planes = y.shape
+        Mout, width = y.shape
         w2 = self._packed[name + ".conv2.weight"]
-        if planes % 64 == 0:
+        if width % 64 == 0:
             # implicit GEMM: 4-D TMA boxes gather the taps (zero fill = padding); stride 2 through TMA traversal strides
-            gemm(a1, w2, y, Mout, planes, 9 * planes, lda=planes, conv=(B, Hc, Wc, planes), conv_mode=1,
+            gemm(a1, w2, y, Mout, width, 9 * width, lda=width, conv=(B, Hc, Wc, width), conv_mode=1,
                  conv_stride=stride, **epi)
             return None
-        cols = self.ws.get(key, (Mout, 9 * planes), BF16)
-        call("vtx_im2col3x3", a1.data_ptr(), cols.data_ptr(), B, Hc, Wc, planes, stride, _stream())
-        gemm(cols, w2, y, Mout, planes, 9 * planes, **epi)
+        cols = self.ws.get(key, (Mout, 9 * width), BF16)
+        call("vtx_im2col3x3", a1.data_ptr(), cols.data_ptr(), B, Hc, Wc, width, stride, _stream())
+        gemm(cols, w2, y, Mout, width, 9 * width, **epi)
         return cols
 
     def _downsample(self, name, x, y, B, Hc, Wc, stride, key, **epi):
-        """1x1 shortcut conv (stride) of block `name`: x [B*Hc*Wc, Cin] -> y [Mout, 4*planes]; returns the matrix the
+        """1x1 shortcut conv (stride) of block `name`: x [B*Hc*Wc, Cin] -> y [Mout, C4]; returns the matrix the
         GEMM read (x itself at stride 1, otherwise its subsampled copy), or None when the strided implicit GEMM read x
         in place."""
         Mout, C4 = y.shape
@@ -416,29 +422,28 @@ class Engine:
         Hc, Wc, Cin = Hp, Wp, 64
         # ---- bottleneck blocks
         for name, blk in self.blocks:
-            planes = blk.conv1.weight.shape[0]
+            width, C4 = _block_widths(blk)
             stride = blk.stride
             Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
             Min, Mout = B * Hc * Wc, B * Hn * Wn
-            rec = dict(name=name, x=x, Hin=Hc, Win=Wc, Hout=Hn, Wout=Wn, Cin=Cin, planes=planes, stride=stride,
+            rec = dict(name=name, x=x, Hin=Hc, Win=Wc, Hout=Hn, Wout=Wn, Cin=Cin, width=width, Cout=C4, stride=stride,
                        Min=Min, Mout=Mout, has_ds=blk.downsample is not None)
             # conv1 1x1
-            y1 = ws.get(name + ".y1", (Min, planes), BF16)
-            st1 = self._slab_take(2 * planes) if training else None
-            gemm(x, self.W(name + ".conv1.weight").view(planes, Cin), y1, Min, planes, Cin, stats=st1)
-            a1 = ws.get(name + ".a1", (Min, planes), BF16)
-            bnp1 = self._bn_act_fwd(y1, name + ".bn1", Min, planes, training, st1, a1)
+            y1 = ws.get(name + ".y1", (Min, width), BF16)
+            st1 = self._slab_take(2 * width) if training else None
+            gemm(x, self.W(name + ".conv1.weight").view(width, Cin), y1, Min, width, Cin, stats=st1)
+            a1 = ws.get(name + ".a1", (Min, width), BF16)
+            bnp1 = self._bn_act_fwd(y1, name + ".bn1", Min, width, training, st1, a1)
             # conv2 3x3 (stride)
-            y2 = ws.get(name + ".y2", (Mout, planes), BF16)
-            st2 = self._slab_take(2 * planes) if training else None
+            y2 = ws.get(name + ".y2", (Mout, width), BF16)
+            st2 = self._slab_take(2 * width) if training else None
             rec["cols2"] = self._conv2(name, a1, y2, B, Hc, Wc, stride, name + ".cols2", stats=st2)
-            a2 = ws.get(name + ".a2", (Mout, planes), BF16)
-            bnp2 = self._bn_act_fwd(y2, name + ".bn2", Mout, planes, training, st2, a2)
+            a2 = ws.get(name + ".a2", (Mout, width), BF16)
+            bnp2 = self._bn_act_fwd(y2, name + ".bn2", Mout, width, training, st2, a2)
             # conv3 1x1
-            C4 = 4 * planes
             y3 = ws.get(name + ".y3", (Mout, C4), BF16)
             st3 = self._slab_take(2 * C4) if training else None
-            gemm(a2, self.W(name + ".conv3.weight").view(C4, planes), y3, Mout, C4, planes, stats=st3)
+            gemm(a2, self.W(name + ".conv3.weight").view(C4, width), y3, Mout, C4, width, stats=st3)
             out = ws.get(name + ".out", (Mout, C4), BF16)
             # backward needs only the SIGN of the block output's pre-activation: one bit per element instead of re-reading
             # the bf16 output twice (bn_bwd_reduce and bn_bwd_apply)
@@ -492,20 +497,20 @@ class Engine:
         # ---- bottleneck blocks: four GEMMs, each ending in its BN (+ shortcut) (+ ReLU); block outputs alternate
         # between two buffers
         for bi, (name, blk) in enumerate(self.blocks):
-            planes = blk.conv1.weight.shape[0]
+            width, C4 = _block_widths(blk)
             stride = blk.stride
             Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
-            Min, Mout, C4 = B * Hc * Wc, B * Hn * Wn, 4 * planes
-            a1 = ws.get("inf.a1", (Min, planes), BF16)
-            gemm(x, self.W(name + ".conv1.weight").view(planes, Cin), a1, Min, planes, Cin, act=1, **ss(name + ".bn1"))
-            a2 = ws.get("inf.a2", (Mout, planes), BF16)
+            Min, Mout = B * Hc * Wc, B * Hn * Wn
+            a1 = ws.get("inf.a1", (Min, width), BF16)
+            gemm(x, self.W(name + ".conv1.weight").view(width, Cin), a1, Min, width, Cin, act=1, **ss(name + ".bn1"))
+            a2 = ws.get("inf.a2", (Mout, width), BF16)
             self._conv2(name, a1, a2, B, Hc, Wc, stride, "inf.cols2", act=1, **ss(name + ".bn2"))
             shortcut = x
             if blk.downsample is not None:
                 shortcut = ws.get("inf.shortcut", (Mout, C4), BF16)
                 self._downsample(name, x, shortcut, B, Hc, Wc, stride, "inf.xs", **ss(name + ".downsample.1"))
             out = ws.get(f"inf.x{bi & 1}", (Mout, C4), BF16)
-            gemm(a2, self.W(name + ".conv3.weight").view(C4, planes), out, Mout, C4, planes, residual=shortcut, act=1,
+            gemm(a2, self.W(name + ".conv3.weight").view(C4, width), out, Mout, C4, width, residual=shortcut, act=1,
                  **ss(name + ".bn3"))
             x, Hc, Wc, Cin = out, Hn, Wn, C4
         return x, Hc, Wc
@@ -563,14 +568,14 @@ class Engine:
         sums3 = None  # bn3 sums of the current block when the GEMM that produced dOut already accumulated them
         for bi in range(len(blocks) - 1, -1, -1):
             rec = blocks[bi]
-            name, planes, Cin, stride = rec["name"], rec["planes"], rec["Cin"], rec["stride"]
+            name, width, Cin, stride = rec["name"], rec["width"], rec["Cin"], rec["stride"]
             layer = name.split(".")[2]
             if prev_layer is not None and layer != prev_layer:
                 self._run_jobs("unpack:" + prev_layer, lambda: self._unpack_rows(prev_layer, stem_s2d))
                 if bucket_cb is not None:
                     bucket_cb(prev_layer)
             prev_layer = layer
-            Min, Mout, C4 = rec["Min"], rec["Mout"], 4 * rec["planes"]
+            Min, Mout, C4 = rec["Min"], rec["Mout"], rec["Cout"]
             Hc, Wc, Hn, Wn = rec["Hin"], rec["Win"], rec["Hout"], rec["Wout"]
             # ---- block output: ReLU mask + bn3 (+ downsample BN) backward
             dy3 = ws.get("bwd.dy3", (Mout, C4), BF16)
@@ -586,33 +591,33 @@ class Engine:
                 self._bn_bwd(dOut, rec["m3"], rec["y3"], rec["bnp3"], name + ".bn3", Mout, C4, dy3, sums=sums3)
             sums3 = None
             # ---- conv3 (1x1): wgrad + dgrad; the dgrad epilogue accumulates bn2's backward sums (ReLU mask from y2)
-            self._wgrad(dy3, rec["a2"], self.G(name + ".conv3.weight"), C4, planes, Mout)
-            da2 = ws.get("bwd.da2", (Mout, planes), BF16)
-            sums2 = self._slab_take(2 * planes)
-            gemm(dy3, self.W(name + ".conv3.weight").view(C4, planes), da2, Mout, planes, C4, b_mn=1,
+            self._wgrad(dy3, rec["a2"], self.G(name + ".conv3.weight"), C4, width, Mout)
+            da2 = ws.get("bwd.da2", (Mout, width), BF16)
+            sums2 = self._slab_take(2 * width)
+            gemm(dy3, self.W(name + ".conv3.weight").view(C4, width), da2, Mout, width, C4, b_mn=1,
                  bnr=(rec["y2"], rec["bnp2"], sums2, None))
             # ---- bn2 + ReLU backward
-            dy2 = ws.get("bwd.dy2", (Mout, planes), BF16)
-            self._bn_bwd(da2, None, rec["y2"], rec["bnp2"], name + ".bn2", Mout, planes, dy2, mask_from_y=1, sums=sums2)
+            dy2 = ws.get("bwd.dy2", (Mout, width), BF16)
+            self._bn_bwd(da2, None, rec["y2"], rec["bnp2"], name + ".bn2", Mout, width, dy2, mask_from_y=1, sums=sums2)
             # ---- conv2 (3x3): wgrad + dgrad
-            dwp = self._dwp[name + ".conv2"].view(planes, 9 * planes)
-            da1 = ws.get("bwd.da1", (Min, planes), BF16)
+            dwp = self._dwp[name + ".conv2"].view(width, 9 * width)
+            da1 = ws.get("bwd.da1", (Min, width), BF16)
             sums1 = None
             if rec["cols2"] is None:
-                if planes == 64 and stride == 1:
+                if width == 64 and stride == 1:
                     # wgrad in the [(tap, cin), cout] layout (vtx_conv_w_unpack_add_t folds it into OIHW)
-                    gemm(dy2, rec["a1"], dwp, 9 * planes, planes, Mout, atomic=True, lda=planes, ldb=planes, ldd=planes,
-                         conv=(B, Hc, Wc, planes), conv_mode=4, out_f32=True)
+                    gemm(dy2, rec["a1"], dwp, 9 * width, width, Mout, atomic=True, lda=width, ldb=width, ldd=width,
+                         conv=(B, Hc, Wc, width), conv_mode=4, out_f32=True)
                 else:
-                    tiles = ((planes + 127) // 128) * ((9 * planes + 255) // 256)
+                    tiles = ((width + 127) // 128) * ((9 * width + 255) // 256)
                     sk = ops.split_k_for(tiles, (Mout + 63) // 64)
-                    gemm(dy2, rec["a1"], dwp, planes, 9 * planes, Mout, atomic=True, split_k=sk, lda=planes,
-                         ldb=planes, conv=(B, Hc, Wc, planes), conv_mode=2, out_f32=True, conv_stride=stride)
+                    gemm(dy2, rec["a1"], dwp, width, 9 * width, Mout, atomic=True, split_k=sk, lda=width,
+                         ldb=width, conv=(B, Hc, Wc, width), conv_mode=2, out_f32=True, conv_stride=stride)
                 if stride in (1, 2):
-                    sums1 = self._slab_take(2 * planes)  # bn1's backward sums, accumulated by the conv2-dgrad epilogue(s)
+                    sums1 = self._slab_take(2 * width)  # bn1's backward sums, accumulated by the conv2-dgrad epilogue(s)
                 if stride == 1:
-                    gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Min, planes, 9 * planes, lda=planes,
-                         conv=(B, Hc, Wc, planes), conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
+                    gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Min, width, 9 * width, lda=width,
+                         conv=(B, Hc, Wc, width), conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
                 elif stride == 2:
                     # strided dgrad as four implicit GEMMs, one per parity class (ph, pw) of the input position: row
                     # 2i+ph of da1 gathers dy rows i+a, a < 1+ph, through kernel rows ph+1-2a (same along w); each class
@@ -624,29 +629,29 @@ class Engine:
                             Hs, Ws = (Hc - ph + 1) // 2, (Wc - pw + 1) // 2
                             if Hs <= 0 or Ws <= 0:
                                 continue
-                            voff = (ph * Wc + pw) * planes * 2
-                            gemm(dy2, self._packed[f"{name}.conv2.weight#dgrad_s2_{ph}{pw}"], da1, Mout, planes,
-                                 th * tw * planes, lda=planes, conv=(B, Hn, Wn, planes), conv_mode=1, tap_grid=(th, tw, 0),
+                            voff = (ph * Wc + pw) * width * 2
+                            gemm(dy2, self._packed[f"{name}.conv2.weight#dgrad_s2_{ph}{pw}"], da1, Mout, width,
+                                 th * tw * width, lda=width, conv=(B, Hn, Wn, width), conv_mode=1, tap_grid=(th, tw, 0),
                                  d_ptr=da1.data_ptr() + voff,
-                                 out_view=(Hs, Ws, 2 * planes, 2 * Wc * planes, Hc * Wc * planes),
+                                 out_view=(Hs, Ws, 2 * width, 2 * Wc * width, Hc * Wc * width),
                                  bnr=(rec["y1"], rec["bnp1"], sums1, None, rec["y1"].data_ptr() + voff))
                 else:  # other strides: per-tap gradients by a plain GEMM, scattered back by col2im
-                    dcols = ws.get("bwd.dcols", (Mout, 9 * planes), BF16)
-                    gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * planes, planes, b_mn=1)
-                    call("vtx_col2im3x3", dcols.data_ptr(), da1.data_ptr(), B, Hc, Wc, planes, stride, s)
+                    dcols = ws.get("bwd.dcols", (Mout, 9 * width), BF16)
+                    gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * width, width, b_mn=1)
+                    call("vtx_col2im3x3", dcols.data_ptr(), da1.data_ptr(), B, Hc, Wc, width, stride, s)
             else:
-                self._wgrad(dy2, rec["cols2"], dwp, planes, 9 * planes, Mout)
-                dcols = ws.get("bwd.dcols", (Mout, 9 * planes), BF16)
-                gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * planes, planes, b_mn=1)
-                call("vtx_col2im3x3", dcols.data_ptr(), da1.data_ptr(), B, Hc, Wc, planes, stride, s)
+                self._wgrad(dy2, rec["cols2"], dwp, width, 9 * width, Mout)
+                dcols = ws.get("bwd.dcols", (Mout, 9 * width), BF16)
+                gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * width, width, b_mn=1)
+                call("vtx_col2im3x3", dcols.data_ptr(), da1.data_ptr(), B, Hc, Wc, width, stride, s)
             # ---- bn1 + ReLU backward
-            dy1 = ws.get("bwd.dy1", (Min, planes), BF16)
-            self._bn_bwd(da1, None, rec["y1"], rec["bnp1"], name + ".bn1", Min, planes, dy1, mask_from_y=1, sums=sums1)
+            dy1 = ws.get("bwd.dy1", (Min, width), BF16)
+            self._bn_bwd(da1, None, rec["y1"], rec["bnp1"], name + ".bn1", Min, width, dy1, mask_from_y=1, sums=sums1)
             # ---- conv1 (1x1): wgrad + dgrad (+ shortcut gradient)
-            self._wgrad(dy1, rec["x"], self.G(name + ".conv1.weight"), planes, Cin, Min)
+            self._wgrad(dy1, rec["x"], self.G(name + ".conv1.weight"), width, Cin, Min)
             dx = ws.get(f"bwd.dx{scratch_i & 1}", (Min, Cin), BF16)
             scratch_i += 1
-            w1 = self.W(name + ".conv1.weight").view(planes, Cin)
+            w1 = self.W(name + ".conv1.weight").view(width, Cin)
             if rec["has_ds"]:
                 wd = self.W(name + ".downsample.0.weight").view(C4, Cin)
                 if rec["xs"] is not None:
@@ -656,7 +661,7 @@ class Engine:
                     gemm(dyd, rec["x"], self.G(name + ".downsample.0.weight").view(C4, Cin), C4, Cin, Mout, atomic=True,
                          split_k=ops.split_k_for(tiles, (Mout + 63) // 64), lda=C4, ldb=Cin, conv=(B, Hc, Wc, Cin),
                          conv_mode=2, conv_stride=stride, conv_taps=1, out_f32=True)
-                gemm(dy1, w1, dx, Min, Cin, planes, b_mn=1)
+                gemm(dy1, w1, dx, Min, Cin, width, b_mn=1)
                 if stride == 1:
                     gemm(dyd, wd, dx, Min, Cin, C4, b_mn=1, residual=dx)
                 elif stride == 2 and rec["xs"] is None:
@@ -677,7 +682,7 @@ class Engine:
                 if prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
                     sums3 = self._slab_take(2 * Cin)
                     bnr3 = (prev["y3"], prev["bnp3"], sums3, prev["m3"])
-                gemm(dy1, w1, dx, Min, Cin, planes, b_mn=1, residual=dOut, residual_mask=rec["m3"], bnr=bnr3)
+                gemm(dy1, w1, dx, Min, Cin, width, b_mn=1, residual=dOut, residual_mask=rec["m3"], bnr=bnr3)
             dOut = dx
         # ---- stem: maxpool bwd -> ReLU/BN bwd -> wgrad
         st = tape["stem"]

@@ -13,7 +13,10 @@ from typing import List, Optional
 import torch
 from torch import nn
 
-_RESNET_BLOCKS = {"resnet50": [3, 4, 6, 3], "resnet101": [3, 4, 23, 3], "resnet152": [3, 8, 36, 3]}
+# torchvision ResNet name -> (bottleneck blocks per layer, width_per_group).  A bottleneck of `planes` has inner width
+# planes * width_per_group / 64 and output width 4 * planes (torchvision/models/resnet.py:108-163, groups = 1).
+_RESNET_ARCHS = {"resnet50": ([3, 4, 6, 3], 64), "resnet101": ([3, 4, 23, 3], 64), "resnet152": ([3, 8, 36, 3], 64),
+                 "wide_resnet50_2": ([3, 4, 6, 3], 128), "wide_resnet101_2": ([3, 4, 23, 3], 128)}
 
 
 class _NoForward(nn.Module):
@@ -22,16 +25,19 @@ class _NoForward(nn.Module):
 
 
 class Bottleneck(_NoForward):
-    """Parameters of torchvision's Bottleneck (torchvision/models/resnet.py:108-163): 1x1 -> 3x3(stride) -> 1x1."""
+    """Parameters of torchvision's Bottleneck (torchvision/models/resnet.py:108-163): 1x1 -> 3x3(stride) -> 1x1.
+    `width` is the inner width of conv1 / conv2 (torchvision: planes * width_per_group / 64; `planes` when None)."""
     expansion = 4
 
-    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: bool = False):
+    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: bool = False,
+                 width: Optional[int] = None):
         super().__init__()
-        self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
-        self.bn1 = nn.BatchNorm2d(planes)
-        self.conv2 = nn.Conv2d(planes, planes, 3, stride=stride, padding=1, bias=False)
-        self.bn2 = nn.BatchNorm2d(planes)
-        self.conv3 = nn.Conv2d(planes, planes * 4, 1, bias=False)
+        width = planes if width is None else width
+        self.conv1 = nn.Conv2d(inplanes, width, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(width)
+        self.conv2 = nn.Conv2d(width, width, 3, stride=stride, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(width)
+        self.conv3 = nn.Conv2d(width, planes * 4, 1, bias=False)
         self.bn3 = nn.BatchNorm2d(planes * 4)
         self.stride = stride
         self.downsample = None
@@ -41,7 +47,8 @@ class Bottleneck(_NoForward):
 
 
 class ResNetParams(_NoForward):
-    """Parameter tree of torchvision ResNet-50/101/152 up to layer4 (`fc` replaced by Identity as in the reference).
+    """Parameter tree of torchvision ResNet-50/101/152 and Wide ResNet-50-2/101-2 up to layer4 (`fc` replaced by
+    Identity as in the reference).  Every one ends in 2048 channels.
 
     Callable like torchvision's ResNet (the downstream evaluations, scripts/clf_linear.py and scripts/clf_voc07.py):
     `forward(image fp32 (B,3,H,W)) -> fc(flatten(avgpool(layer4)))` in fp32, the (B, 2048) pooled features while `fc`
@@ -52,9 +59,10 @@ class ResNetParams(_NoForward):
 
     def __init__(self, name: str = "resnet50", zero_init_residual: bool = True):
         super().__init__()
-        if name not in _RESNET_BLOCKS:
-            raise KeyError(f"unsupported torchvision backbone '{name}' (supported: {sorted(_RESNET_BLOCKS)})")
-        self.blocks_per_layer: List[int] = list(_RESNET_BLOCKS[name])
+        if name not in _RESNET_ARCHS:
+            raise KeyError(f"unsupported torchvision backbone '{name}' (supported: {sorted(_RESNET_ARCHS)})")
+        blocks_per_layer, width_per_group = _RESNET_ARCHS[name]
+        self.blocks_per_layer: List[int] = list(blocks_per_layer)
         self.conv1 = nn.Conv2d(3, 64, 7, stride=2, padding=3, bias=False)
         self.bn1 = nn.BatchNorm2d(64)
         inplanes = 64
@@ -62,7 +70,8 @@ class ResNetParams(_NoForward):
             blocks = []
             for bi in range(n):
                 stride = 2 if (bi == 0 and li > 1) else 1
-                blocks.append(Bottleneck(inplanes, planes, stride, downsample=(stride != 1 or inplanes != planes * 4)))
+                blocks.append(Bottleneck(inplanes, planes, stride, downsample=(stride != 1 or inplanes != planes * 4),
+                                         width=planes * width_per_group // 64))
                 inplanes = planes * 4
             setattr(self, f"layer{li}", nn.Sequential(*blocks))
         self.avgpool = nn.AdaptiveAvgPool2d((1, 1))  # torchvision's attribute (no state); forward pools in CUDA
