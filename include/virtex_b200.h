@@ -44,6 +44,8 @@ int vtx_num_sms(void);
  * Epilogue order: acc -> (stats: per-column sum / sum of squares of acc, fp32 atomics) -> *alpha -> +bias[n]
  *                 -> +residual[m,n] (bf16) -> activation -> store (bf16 or fp32; or fp32 atomic accumulate).
  * split_k > 1 requires atomic = 1 (fp32 output, caller zero-initialises).
+ * A bf16 output is stored by the TMA unit in 16-byte chunks: when N % 8 != 0, columns N .. round_up(N, 8) - 1 of every
+ * output row are overwritten too, so D's rows must own that padding.
  * ------------------------------------------------------------------------------------------------------------------ */
 typedef struct VtxGemm {
   const void* A;
