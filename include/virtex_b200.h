@@ -298,6 +298,20 @@ int vtx_beam_rows(const float* logits, int64_t ldl, int R, int V, const int64_t*
 int vtx_beam_select(const float* cand_val, const int32_t* cand_idx, int parents, int k, int beam, const float* scores_in,
                     float* scores_out, int32_t* parent_out, const int64_t* pred_in, int64_t* pred_out,
                     const int32_t* index_in, int32_t* index_out, int B, int s, int eos, int32_t* alive, void* stream);
+/* One step of nucleus sampling (AutoRegressiveNucleusSampling, virtex/utils/nucleus_sampling.py:58-115), one row of
+   fp32 logits [R, ldl] (V columns) per CTA, last token last[row].  In (descending value, ascending column) order, with
+   fp32 probabilities from a one-pass log-sum-exp, the nucleus keeps every token whose preceding cumulative probability
+   is <= p (the first token always); the last token is then banned, and the new token is drawn from the softmax of
+   the remaining nucleus by the inverse CDF in ascending column order at the uniform
+       u = (hash_u64(*seed, 4000, s * R + row) >> 40) / 2^24        (vtx_common.cuh; 24 bits, exact in fp32).
+   When the nucleus is the last token alone, every logit is -1e12 in the reference and the draw is uniform over all
+   V tokens: floor(u * V).  A row whose last token is eos draws eos.  Writes pred[s * R + row] of the step-major int64
+   table [steps, R] and sets alive[s] = 1 if the new token is not eos (alive is zeroed by the caller).  Cumulative
+   masses are fixed-point integers: bitwise deterministic for a seed.  The seed is read on the device, so a captured
+   launch stays valid.  0 <= p <= 1, V <= VTX_NUCLEUS_MAX_V (the row is staged in shared memory). */
+#define VTX_NUCLEUS_MAX_V 32768
+int vtx_nucleus_sample(const float* logits, int64_t ldl, int R, int V, const int64_t* last, int eos, float p,
+                       const uint64_t* seed, int s, int64_t* pred, int32_t* alive, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * GPU input pipeline (csrc/input_pipe.cu): decoded uint8 HWC images -> fp32 NCHW network input, token lists -> padded

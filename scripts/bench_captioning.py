@@ -1,14 +1,17 @@
 #!/usr/bin/env python
-"""Beam-search captioning throughput: the engine's incremental decoder against the eager-PyTorch incumbent.
+"""Captioning throughput: the engine's incremental decoder against the eager-PyTorch incumbent, by beam search or by
+nucleus sampling.
 
     python scripts/bench_captioning.py --batch 256 --beam 5 --max-steps 30 --heads L1_H1024 L4_H1024 L1_H2048
+    python scripts/bench_captioning.py --decoder nucleus_sampling --nucleus-size 0.9
 
 Setting of scripts/eval_captioning.py: batch 256, 224 x 224 images, beam 5 (per-node 2), 30 decoding steps; random-init
 weights with the EOS column of `textual.output.bias` at -30 so that both paths run all 30 steps.  Engine: image ->
 tokens through `model({"image": x})` (backbone with folded BN, one decoder position per step over the cache).
 Incumbent, alternating with the engine in the same process: torchvision resnet50 + scripts/gpu_incumbent.py's `Head`
 under bf16 autocast, eval mode, recomputing the whole prefix every step, with the search's rules vectorised (the
-repetition penalty as one scatter).  Prints one JSON line per head with the card's name and power limit; decode FLOPs
+repetition penalty as one scatter); for nucleus sampling, the reference's rules (SOS-prefixed prefix, sort + cumsum
+nucleus, last-token ban, multinomial draw) on whole batches.  Prints one JSON line per head with the card's name and power limit; decode FLOPs
 are counted from the shapes (GEMMs and attention; the backbone separately).  `--profile` adds one torch.profiler run of
 the engine per head, reporting the share of the decode span in which no kernel of the run was executing.
 """
@@ -37,11 +40,11 @@ def card():
     return q or torch.cuda.get_device_name(0)
 
 
-def decode_flops(B, beam, steps, L, H, Sk=49, Cv=2048):
+def decode_flops(B, beam, steps, L, H, Sk=49, Cv=2048, sampler=False):
     """FLOPs of the incremental decode (everything after the backbone), from the shapes."""
     f = 2 * B * Sk * Cv * H + L * 2 * B * Sk * H * 2 * H  # visual projection, cross-attention K|V
     for t in range(steps):
-        rows, keys = (B, 1) if t == 0 else (B * beam, t)
+        rows, keys = (B, t + 1) if sampler else (B, 1) if t == 0 else (B * beam, t)
         per_layer = 2 * rows * H * (3 * H + H + H + H + 8 * H) + 4 * rows * H * (keys + Sk)
         f += L * per_layer + 2 * rows * H * V
     return f
@@ -56,13 +59,13 @@ def build(L, H, B):
 
 
 class Incumbent:
-    def __init__(self, L, H, beam, steps):
+    def __init__(self, L, H, beam, steps, nucleus_size=None):
         self.cnn = torchvision.models.resnet50(weights=None).cuda().eval()
         self.cnn.fc = torch.nn.Identity()
         self.head = Head(2048, V, H, L, H // 64, 4 * H, 0.1).cuda().eval()
         with torch.no_grad():
             self.head.output.bias[EOS] = -30.0
-        self.beam, self.steps = beam, steps
+        self.beam, self.steps, self.nucleus_size = beam, steps, nucleus_size
 
     @torch.no_grad()
     def __call__(self, image):
@@ -79,6 +82,8 @@ class Incumbent:
                 lengths = torch.full((tokens.shape[0],), tokens.shape[1], device=tokens.device)
                 return self.head(feats, tokens, lengths)[:, -1].float()
 
+            if self.nucleus_size is not None:
+                return self._sample(step, B, image.device)
             lp = F.log_softmax(step(torch.full((B, 1), SOS, device=image.device)), 1)
             scores, tok = lp.topk(beam)
             pred = tok.reshape(B * beam, 1)
@@ -100,6 +105,25 @@ class Incumbent:
                 pred = torch.cat([pred[parent], i.view(B, beam * 2).gather(1, sel).reshape(-1, 1)], 1)
                 scores = best.reshape(-1)
             return pred[::beam]
+
+    def _sample(self, step, B, device):
+        pred = torch.full((B, 1), SOS, device=device)
+        rows = torch.arange(B, device=device)
+        for _ in range(self.steps):
+            last = pred[:, -1]
+            if bool((last == EOS).all()):
+                break
+            logits = step(pred)
+            sorted_logits, sorted_idx = torch.sort(logits, descending=True)
+            remove = torch.cumsum(F.softmax(sorted_logits, -1), -1) > self.nucleus_size
+            remove[:, 1:] = remove[:, :-1].clone()
+            remove[:, 0] = False
+            logits[remove.scatter(1, sorted_idx, remove)] = -1e12
+            logits[rows, last] = -1e12
+            tok = torch.multinomial(F.softmax(logits, -1), 1).view(B)
+            tok[last == EOS] = EOS
+            pred = torch.cat([pred, tok[:, None]], 1)
+        return pred[:, 1:]
 
 
 def timed(fn, reps):
@@ -148,21 +172,30 @@ def main():
     ap.add_argument("--heads", nargs="+", default=["L1_H1024", "L4_H1024", "L1_H2048"])
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--decoder", choices=["beam_search", "nucleus_sampling"], default="beam_search")
+    ap.add_argument("--nucleus-size", type=float, default=0.9)
     a = ap.parse_args()
     from virtex_b200.factories import CaptionDecoderFactory
     from virtex_b200.models import ForwardCaptioningModel
     gpu = card()
     B, beam, steps = a.batch, a.beam, a.max_steps
+    sampler = a.decoder == "nucleus_sampling"
+    if sampler:
+        beam = 1
     image = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(0)).cuda()
     for spec in a.heads:
         L, H = (int(p[1:]) for p in spec.split("_"))
         visual, textual = build(L, H, B)
-        dec = CaptionDecoderFactory.create("beam_search", eos_index=EOS, max_steps=steps, beam_size=beam)
+        if sampler:
+            dec = CaptionDecoderFactory.create("nucleus_sampling", eos_index=EOS, max_steps=steps,
+                                               nucleus_size=a.nucleus_size)
+        else:
+            dec = CaptionDecoderFactory.create("beam_search", eos_index=EOS, max_steps=steps, beam_size=beam)
         model = ForwardCaptioningModel(visual, textual, decoder=dec).cuda().eval()
         with torch.no_grad():
             model.textual.output.bias[EOS] = -30.0
         eng = model.engine
-        inc = Incumbent(L, H, beam, steps)
+        inc = Incumbent(L, H, beam, steps, a.nucleus_size if sampler else None)
         with torch.no_grad():
             out = model({"image": image})["predictions"]
             ref = inc(image)
@@ -174,8 +207,9 @@ def main():
                 t_bb += timed(lambda: eng.backbone_infer(image), 1)
         ms, ms_inc, ms_bb = min(t_eng), min(t_inc), min(t_bb)
         dec_ms = ms - ms_bb
-        fl = decode_flops(B, beam, steps, L, H)
-        row = {"head": spec, "card": gpu, "batch": B, "beam": beam, "steps": steps,
+        fl = decode_flops(B, beam, steps, L, H, sampler=sampler)
+        row = {"head": spec, "card": gpu, "decoder": a.decoder, "batch": B, "beam": beam, "steps": steps,
+               **({"nucleus_size": a.nucleus_size} if sampler else {}),
                "engine_images_s": round(B / ms * 1e3, 1), "engine_ms": [round(t, 2) for t in t_eng],
                "incumbent_images_s": round(B / ms_inc * 1e3, 1), "incumbent_ms": [round(t, 2) for t in t_inc],
                "speedup": round(ms_inc / ms, 2), "backbone_ms": round(ms_bb, 2), "decode_ms": round(dec_ms, 2),

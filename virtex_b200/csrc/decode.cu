@@ -2,8 +2,9 @@
 // single-query attention over a key block per row (self-attention over the growing cache, cross-attention over the
 // image's projected features), and the two halves of one beam step -- per-row log-softmax with the reference's
 // repetition penalty and EOS continuation + per-row top-k, then the per-image selection that also gathers the
-// predictions and the cache index table of the surviving beams.  Everything else of a decoding step is a GEMM or an
-// existing head kernel run with dropout p = 0.
+// predictions and the cache index table of the surviving beams -- and one step of nucleus sampling
+// (virtex/utils/nucleus_sampling.py).  Everything else of a decoding step is a GEMM or an existing head kernel run with
+// dropout p = 0.
 #include "vtx_common.cuh"
 #include "../../include/virtex_b200.h"
 
@@ -218,6 +219,213 @@ __global__ void __launch_bounds__(32 * kSelectWarps) beam_select_kernel(
   if (__any_sync(0xffffffffu, lane < beam && my_tok != eos) && lane == 0) alive[s] = 1;
 }
 
+// ------------------------------------------------------------------------------------------------ nucleus sampling
+// One CTA per row of fp32 logits (AutoRegressiveNucleusSampling.search, nucleus_sampling.py:77-113).  The row is staged
+// once in shared memory; every later pass reads it from there.
+//   1. p_i = exp(x_i - lse) in fp32 (one-pass log-sum-exp), as fixed-point mass q_i = rint(p_i * 2^40): integer sums
+//      are exact, so every cumulative mass below is independent of summation order.
+//   2. The crossing token -- the first token, in (descending value, ascending id) order, whose inclusive cumulative
+//      mass exceeds thr = floor(p * 2^40) -- by a radix select over order-preserving 32-bit value keys, 11 + 11 + 10
+//      bits, with a mass histogram per digit.  Exact ties share one mass, so the crossing tie's rank is arithmetic,
+//      and a scan in id order finds its id.  The nucleus is every token up to and including it (all tokens when the
+//      whole mass is <= thr).
+//   3. The row's last token is banned after the nucleus is chosen.  The sample is the inverse CDF, in ascending id,
+//      of the weights rint(exp(x_i - m) * 2^40) of the kept unbanned tokens (m: their largest logit), at the uniform
+//      u = (hash_u64(seed, kNucleusSite, s * R + row) >> 40) / 2^24; when the nucleus is the last token alone, the
+//      reference's softmax over all -1e12 logits is uniform: token floor(u * V).
+// Tokens of mass below 2^-41 (nucleus) or weight below 2^-41 of the largest (sampling) round to zero and are never
+// drawn; the reference draws them with probability below 1e-12.
+constexpr int kNucThreads = 256;
+constexpr int kNucBins = 2048;
+constexpr uint32_t kNucleusSite = 4000u;  // hash site of the sampler's uniforms; dropout sites are below 2000
+
+// ascending key = descending value (the logits are NaN-free and -0 is +0 by now)
+__device__ __forceinline__ uint32_t nuc_key(float x) {
+  const uint32_t u = __float_as_uint(x);
+  return (u & 0x80000000u) ? u : ~(u | 0x80000000u);
+}
+__device__ __forceinline__ float nuc_value(uint32_t key) {
+  return __uint_as_float((key & 0x80000000u) ? key : (~key & 0x7fffffffu));
+}
+__device__ __forceinline__ unsigned long long nuc_fixed(float x, float ref) {
+  return __float2ull_rn(expf(x - ref) * 0x1p40f);
+}
+
+__device__ __forceinline__ unsigned long long bin_mass(const uint32_t* lo, const uint32_t* hi, int b) {
+  return ((unsigned long long)hi[b] << 32) + lo[b];
+}
+
+// exclusive prefix sum of v over the CTA in thread order; `total` receives the CTA's sum.  scratch: 32 entries.
+__device__ __forceinline__ unsigned long long block_scan_u64(unsigned long long v, unsigned long long* scratch,
+                                                            unsigned long long& total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  unsigned long long inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long n = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += n;
+  }
+  __syncthreads();  // the previous scan's readers of scratch are done
+  if (lane == 31) scratch[warp] = inc;
+  __syncthreads();
+  unsigned long long base = 0;
+  total = 0;
+  for (int w = 0; w < nwarps; ++w) {
+    if (w < warp) base += scratch[w];
+    total += scratch[w];
+  }
+  return base + inc - v;
+}
+
+__global__ void __launch_bounds__(kNucThreads) nucleus_sample_kernel(const float* __restrict__ X, long long ld, int V,
+                                                                     const long long* __restrict__ last, int eos,
+                                                                     float p, const unsigned long long* __restrict__ seed,
+                                                                     int s, int R, long long* __restrict__ pred,
+                                                                     int* __restrict__ alive) {
+  VTX_PDL_TRIGGER();
+  extern __shared__ float xs[];
+  __shared__ uint32_t hist_lo[kNucBins], hist_hi[kNucBins];  // a 64-bit mass histogram as two native-atomic halves
+  __shared__ unsigned long long scratch[32];
+  __shared__ float sm[32], ss[32];
+  __shared__ unsigned long long sel_before;
+  __shared__ int sel_bin, sel_id;
+  const int row = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const int lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
+  const long long lt = last[row];
+  long long* dst = pred + (long long)s * R + row;
+  if (lt == eos) {  // rule 6: an ended caption continues with EOS
+    if (tid == 0) *dst = eos;
+    return;
+  }
+  const float* x = X + (long long)row * ld;
+  float m = -INFINITY, sum = 0.f;
+  for (int i = tid; i < V; i += nt) {
+    float v = x[i];
+    if (isnan(v)) v = -INFINITY;
+    if (v == 0.f) v = 0.f;  // -0 ties with +0, as in a sort by value
+    xs[i] = v;
+    lse_merge(m, sum, v, 1.f);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, sum, o);
+    lse_merge(m, sum, m2, s2);
+  }
+  if (lane == 0) { sm[warp] = m; ss[warp] = sum; }
+  __syncthreads();
+  m = -INFINITY;
+  sum = 0.f;
+  for (int w = 0; w < nwarps; ++w) lse_merge(m, sum, sm[w], ss[w]);
+  const float lse = m + logf(sum);
+
+  // ---- the crossing token's value key: three radix digits, most significant first
+  const unsigned long long thr = (unsigned long long)((double)p * 0x1p40);
+  uint32_t prefix = 0, pmask = 0;
+  unsigned long long before = 0;  // mass of every token whose key is below the current prefix
+  bool all_kept = false;
+  for (int pass = 0; pass < 3; ++pass) {
+    const int shift = pass == 0 ? 21 : pass == 1 ? 10 : 0;
+    const int nb = pass == 2 ? 1024 : 2048;
+    for (int b = tid; b < nb; b += nt) hist_lo[b] = hist_hi[b] = 0;
+    __syncthreads();
+    for (int i = tid; i < V; i += nt) {
+      const float v = xs[i];
+      const uint32_t k = nuc_key(v);
+      if ((k & pmask) == prefix) {
+        const unsigned long long q = nuc_fixed(v, lse);
+        if (q) {  // 64-bit add from two 32-bit atomics (a shared 64-bit atomic add is a compare-and-swap loop)
+          const int b = (k >> shift) & (nb - 1);
+          const uint32_t ql = (uint32_t)q, old = atomicAdd(&hist_lo[b], ql);
+          const uint32_t qh = (uint32_t)(q >> 32) + (old + ql < old ? 1u : 0u);
+          if (qh) atomicAdd(&hist_hi[b], qh);
+        }
+      }
+    }
+    __syncthreads();
+    const int per = nb / nt;
+    unsigned long long local = 0;
+    for (int j = 0; j < per; ++j) local += bin_mass(hist_lo, hist_hi, tid * per + j);
+    unsigned long long total;
+    unsigned long long run = before + block_scan_u64(local, scratch, total);
+    if (pass == 0 && total <= thr) {  // no token crosses p: the nucleus is the whole vocabulary
+      all_kept = true;
+      break;
+    }
+    for (int j = 0; j < per; ++j) {
+      const unsigned long long h = bin_mass(hist_lo, hist_hi, tid * per + j);
+      if (run <= thr && run + h > thr) { sel_bin = tid * per + j; sel_before = run; }
+      run += h;
+    }
+    __syncthreads();
+    prefix |= (uint32_t)sel_bin << shift;
+    pmask |= (uint32_t)(nb - 1) << shift;
+    before = sel_before;
+  }
+
+  // ---- the crossing token's id: tie rank j = floor((thr - before) / q*) among the tokens of key `prefix`, in id order.
+  // The same pass takes the largest logit among the kept unbanned tokens of smaller key.
+  const uint32_t vkey = all_kept ? 0xffffffffu : prefix;  // no token has key 0xffffffff (a NaN)
+  const float vstar = nuc_value(vkey);
+  const unsigned long long rank = all_kept ? 0 : (thr - before) / nuc_fixed(vstar, lse);
+  const int chunk = (V + nt - 1) / nt;
+  const int lo = min(V, tid * chunk), hi = min(V, lo + chunk);
+  unsigned long long ties = 0;
+  float mk = -INFINITY;
+  for (int i = lo; i < hi; ++i) {
+    const uint32_t k = nuc_key(xs[i]);
+    if (k == vkey) ++ties;
+    else if (k < vkey && i != lt) mk = fmaxf(mk, xs[i]);
+  }
+  unsigned long long nties;
+  const unsigned long long tie0 = block_scan_u64(ties, scratch, nties);
+  if (!all_kept && tie0 <= rank && rank < tie0 + ties) {
+    unsigned long long r = tie0;
+    for (int i = lo; i < hi; ++i)
+      if (nuc_key(xs[i]) == vkey && r++ == rank) { sel_id = i; break; }
+  }
+  mk = warp_max(mk);
+  if (lane == 0) sm[warp] = mk;
+  __syncthreads();
+  const int cid = all_kept ? 0x7fffffff : sel_id;
+  mk = -INFINITY;
+  for (int w = 0; w < nwarps; ++w) mk = fmaxf(mk, sm[w]);
+  if (!all_kept) {  // the kept ties are the rank + 1 first ones; the last token may be one of them
+    const bool last_is_kept_tie = lt >= 0 && lt < V && nuc_key(xs[lt]) == vkey && lt <= cid;
+    if (rank + 1 > (last_is_kept_tie ? 1ull : 0ull)) mk = fmaxf(mk, vstar);
+  }
+
+  // ---- inverse CDF over the kept unbanned tokens in ascending id
+  const uint32_t u24 = (uint32_t)(hash_u64(*seed, kNucleusSite, (unsigned long long)s * R + row) >> 40);
+  long long tok;
+  if (mk == -INFINITY) {  // the nucleus is the banned token alone: uniform over the vocabulary
+    tok = (long long)(((unsigned long long)u24 * (unsigned long long)V) >> 24);
+    if (tid == 0) *dst = tok;
+  } else {
+    unsigned long long wsum = 0;
+    for (int i = lo; i < hi; ++i) {
+      const uint32_t k = nuc_key(xs[i]);
+      if (i != lt && (k < vkey || (k == vkey && i <= cid))) wsum += nuc_fixed(xs[i], mk);
+    }
+    unsigned long long W;
+    const unsigned long long w0 = block_scan_u64(wsum, scratch, W);
+    // target = floor(W * u24 / 2^24) < W (W < 2^56, so the product needs 128 bits)
+    const unsigned long long target = (__umul64hi(W, u24) << 40) | ((W * u24) >> 24);
+    tok = -1;
+    if (w0 <= target && target < w0 + wsum) {
+      unsigned long long run = w0;
+      for (int i = lo; i < hi; ++i) {
+        const uint32_t k = nuc_key(xs[i]);
+        if (i != lt && (k < vkey || (k == vkey && i <= cid))) {
+          run += nuc_fixed(xs[i], mk);
+          if (run > target) { tok = i; break; }
+        }
+      }
+      *dst = tok;
+    }
+  }
+  if (tok >= 0 && tok != eos) alive[s] = 1;
+}
+
 }  // namespace vtx
 
 using namespace vtx;
@@ -261,4 +469,17 @@ extern "C" int vtx_beam_select(const float* cand_val, const int32_t* cand_idx, i
       cand_val, cand_idx, parents, k, beam, scores_in, scores_out, parent_out, (const long long*)pred_in,
       (long long*)pred_out, index_in, index_out, B, s, eos, alive);
   return check_launch("beam_select");
+}
+
+extern "C" int vtx_nucleus_sample(const float* logits, int64_t ldl, int R, int V, const int64_t* last, int eos,
+                                  float p, const uint64_t* seed, int s, int64_t* pred, int32_t* alive, void* stream) {
+  REQ(logits && last && seed && pred && alive && R > 0 && V > 0 && ldl >= V && s >= 0, "bad arguments");
+  REQ(V <= VTX_NUCLEUS_MAX_V, "needs V <= VTX_NUCLEUS_MAX_V (32768)");
+  REQ(p >= 0.f && p <= 1.f, "needs 0 <= p <= 1");
+  const int smem = V * (int)sizeof(float);
+  cudaFuncSetAttribute(nucleus_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  nucleus_sample_kernel<<<R, kNucThreads, smem, STREAM>>>(logits, ldl, V, (const long long*)last, eos, p,
+                                                          (const unsigned long long*)seed, s, R, (long long*)pred,
+                                                          alive);
+  return check_launch("nucleus_sample");
 }

@@ -1113,32 +1113,11 @@ class Engine:
         """Backbone (folded BN), visual projection, cross-attention K|V of every layer, and step 0 -> the search
         state (_BeamState) after its first step."""
         mod = self.textual
-        if max_steps - 1 > mod.max_caption_length:
-            raise ValueError(f"max_steps {max_steps} needs {max_steps - 1} positions; the head has "
-                             f"{mod.max_caption_length}")
-        # vtx_attn_decode attends over at most DECODE_MAX_KEYS keys: the max_steps - 1 cache slots of self-attention
-        # and the h * w feature positions of cross-attention (h = w = 8 for a 256 x 256 image)
-        h, w = image.shape[2], image.shape[3]
-        for _ in range(5):  # stem conv, max-pool, layer2..4: each (x - 1) // 2 + 1
-            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-        if max_steps - 1 > DECODE_MAX_KEYS or h * w > DECODE_MAX_KEYS:
-            raise ValueError(f"beam search attends over at most {DECODE_MAX_KEYS} keys: max_steps {max_steps} needs "
-                             f"{max_steps - 1}, a {image.shape[2]} x {image.shape[3]} image {h * w} feature positions")
-        self.mark_weights_dirty()  # parameters may have been updated by any optimiser since the last call
-        feat, h, w = self.backbone_infer(image)
-        B, Sk, ws = image.shape[0], h * w, self.ws
+        Sk, ckv = self._decode_prologue(image, max_steps - 1, "beam search", "bs.")
+        B, ws = image.shape[0], self.ws
         H, V, R = mod.hidden_size, mod.vocab_size, B * beam_size
-        mem = ws.get("bs.mem", (B * Sk, H), BF16)
-        gemm(feat, self.W("textual.visual_projection.weight"), mem, B * Sk, H, feat.shape[1],
-             bias=self.P("textual.visual_projection.bias"))
-        ckv = []
-        for l in range(mod.num_layers):
-            q = f"textual.transformer.layers.{l}.multihead_attn."
-            kv = ws.get(f"bs.ckv{l}", (B * Sk, 2 * H), BF16)
-            gemm(mem, self.W(q + "in_proj_weight")[H:], kv, B * Sk, 2 * H, H, bias=self.P(q + "in_proj_bias")[H:])
-            ckv.append(kv)
         st = _BeamState(B=B, beam=beam_size, per_node=per_node, max_steps=max_steps, eos=eos, R=R, Sk=Sk, ckv=ckv, L=1,
-                        cur=0)
+                        cur=0, pre="bs.")
         st.cache = [ws.get(f"bs.cache{l}", (R, max_steps - 1, 2 * H), BF16) for l in range(mod.num_layers)]
         st.cache0 = [ws.get(f"bs.cache0.{l}", (B, 1, 2 * H), BF16) for l in range(mod.num_layers)]
         st.pred = [ws.get(f"bs.pred{i}", (max_steps, R), torch.int64) for i in (0, 1)]
@@ -1153,6 +1132,35 @@ class Engine:
         self._decode_position(st, B, sos_t, 0, 1, st.cache0, None)
         self._beam_select(st, B, None, beam_size, 1, 0)
         return st
+
+    def _decode_prologue(self, image, positions, what, pre):
+        """Checks that a decoder of `positions` self-attention positions fits the head and the attention kernel (before
+        any launch), then runs the backbone (folded BN), the visual projection and the cross-attention K|V of every
+        layer into workspace keys under `pre` -> (Sk feature positions per image, [bf16 (B * Sk, 2H)] per layer)."""
+        mod = self.textual
+        if positions > mod.max_caption_length:
+            raise ValueError(f"{what} needs {positions} positions; the head has {mod.max_caption_length}")
+        # vtx_attn_decode attends over at most DECODE_MAX_KEYS keys: the self-attention cache slots and the h * w
+        # feature positions of cross-attention (h = w = 8 for a 256 x 256 image)
+        h, w = image.shape[2], image.shape[3]
+        for _ in range(5):  # stem conv, max-pool, layer2..4: each (x - 1) // 2 + 1
+            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        if positions > DECODE_MAX_KEYS or h * w > DECODE_MAX_KEYS:
+            raise ValueError(f"{what} attends over at most {DECODE_MAX_KEYS} keys: it needs {positions} positions, a "
+                             f"{image.shape[2]} x {image.shape[3]} image {h * w} feature positions")
+        self.mark_weights_dirty()  # parameters may have been updated by any optimiser since the last call
+        feat, h, w = self.backbone_infer(image)
+        B, Sk, H = image.shape[0], h * w, mod.hidden_size
+        mem = self.ws.get(pre + "mem", (B * Sk, H), BF16)
+        gemm(feat, self.W("textual.visual_projection.weight"), mem, B * Sk, H, feat.shape[1],
+             bias=self.P("textual.visual_projection.bias"))
+        ckv = []
+        for l in range(mod.num_layers):
+            q = f"textual.transformer.layers.{l}.multihead_attn."
+            kv = self.ws.get(f"{pre}ckv{l}", (B * Sk, 2 * H), BF16)
+            gemm(mem, self.W(q + "in_proj_weight")[H:], kv, B * Sk, 2 * H, H, bias=self.P(q + "in_proj_bias")[H:])
+            ckv.append(kv)
+        return Sk, ckv
 
     def beam_step(self, st):
         """Step t = st.L: decode token t-1 of every beam at position t-1, score, select; st.L becomes t + 1."""
@@ -1176,25 +1184,77 @@ class Engine:
              st.pred[dst].data_ptr(), 0 if src is None else st.index[src].data_ptr(), st.index[dst].data_ptr(), st.B, s,
              st.eos, st.alive.data_ptr(), _stream())
 
+    # ------------------------------------------------------------------------------------------------ nucleus sampling
+    # AutoRegressiveNucleusSampling (virtex/utils/nucleus_sampling.py:47-123) over CaptioningModel.decoding_step, eval
+    # mode, forward-direction head only.  The reference's step t decodes [SOS, tok_1 .. tok_t] (SOS included), so each
+    # step's state is a prefix of the next: step t decodes token t (SOS at t = 0) of every image at position t into
+    # slot t of the image's own cache -- one row per image, no index table, no reordering.  Cross-attention K|V are
+    # projected once per image and layer.  Workspace keys "ns.": a pending backward's tape is left alone, and the
+    # dropout seed of the training step is not touched (the sampler's seed is a buffer of its own).
+    def nucleus_sample(self, image, p, max_steps, sos, eos, seed):
+        """image fp32 NCHW [B,3,H,W] -> int64 (B, L) on the device: one sampled caption per image, EOS repeated after
+        its first EOS; L <= max_steps is the number of steps run before every caption ended in EOS.  `seed`: a Python
+        int or an int64 device tensor of one element (read on the device)."""
+        st = self.nucleus_start(image, p, max_steps, sos, eos, seed)
+        while st.L < max_steps and st.alive[st.L - 1].item():  # one device-to-host read per step
+            self.nucleus_step(st)
+        return st.tokens().contiguous()
+
+    def nucleus_start(self, image, p, max_steps, sos, eos, seed):
+        """Backbone (folded BN), visual projection, cross-attention K|V of every layer, and step 0 (SOS at position 0)
+        -> the sampler state (_NucleusState) after its first step."""
+        if not 0.0 <= p <= 1.0:
+            raise ValueError(f"nucleus size {p} is not in [0, 1]")
+        mod = self.textual
+        Sk, ckv = self._decode_prologue(image, max_steps, "nucleus sampling", "ns.")
+        B, ws = image.shape[0], self.ws
+        H, V = mod.hidden_size, mod.vocab_size
+        st = _NucleusState(B=B, p=float(p), max_steps=max_steps, eos=eos, Sk=Sk, ckv=ckv, L=0, pre="ns.")
+        st.seed = ws.get("ns.seed", (1,), torch.int64)
+        if isinstance(seed, torch.Tensor):
+            st.seed.copy_(seed.reshape(1))
+        else:
+            st.seed.fill_(struct.unpack("<q", struct.pack("<Q", int(seed) & (2 ** 64 - 1)))[0])
+        st.cache = [ws.get(f"ns.cache{l}", (B, max_steps, 2 * H), BF16) for l in range(mod.num_layers)]
+        st.pred = ws.get("ns.pred", (max_steps, B), torch.int64)
+        st.alive = ws.get("ns.alive", (max_steps,), torch.int32)
+        st.alive.zero_()
+        st.logits = ws.get("ns.logits", (B, V), F32)
+        sos_t = ws.get("ns.sos", (B,), torch.int64)
+        sos_t.fill_(sos)
+        self._nucleus_position(st, sos_t)
+        return st
+
+    def nucleus_step(self, st):
+        """Step t = st.L: decode token t of every image at position t, sample token t + 1; st.L becomes t + 1."""
+        self._nucleus_position(st, st.pred[st.L - 1])
+
+    def _nucleus_position(self, st, tokens):
+        t = st.L
+        self._decode_position(st, st.B, tokens, t, 1, st.cache, None)
+        call("vtx_nucleus_sample", st.logits.data_ptr(), st.logits.stride(0), st.B, st.logits.shape[1],
+             tokens.data_ptr(), st.eos, st.p, st.seed.data_ptr(), t, st.pred.data_ptr(), st.alive.data_ptr(), _stream())
+        st.L = t + 1
+
     def _decode_position(self, st, rows, tokens, pos, group, cache, index):
         """Forward head on one new position: tokens int64 [rows] at position `pos`, self-attention over cache slots
         0..pos (slot pos written here; through `index` when given), cross-attention of row m over image m // group
-        -> fp32 logits st.logits[:rows]."""
+        -> fp32 logits st.logits[:rows].  Workspace keys under st.pre."""
         mod = self.textual
         H, A, Fd, V = mod.hidden_size, mod.attention_heads, mod.feedforward_size, mod.vocab_size
-        ws, s, seed = self.ws, _stream(), self.seed.data_ptr()
+        ws, s, seed, k = self.ws, _stream(), self.seed.data_ptr(), st.pre
         emb = "textual.embedding."
-        xs = [ws.get(f"bs.x{i}", (rows, H), F32) for i in (0, 1)]
-        z, zst = ws.get("bs.z", (rows, H), F32), ws.get("bs.st", (rows, 2), F32)
-        xb = ws.get("bs.xb", (rows, H), BF16)
+        xs = [ws.get(f"{k}x{i}", (rows, H), F32) for i in (0, 1)]
+        z, zst = ws.get(k + "z", (rows, H), F32), ws.get(k + "st", (rows, 2), F32)
+        xb = ws.get(k + "xb", (rows, H), BF16)
         # the embedding kernel with T = 1 over position row `pos` is the one-position embedding
         call("vtx_embed_fwd", tokens.data_ptr(), self.P(emb + "words.weight").data_ptr(),
              self.P(emb + "positions.weight")[pos].data_ptr(), self.P(emb + "layer_norm.weight").data_ptr(),
              self.P(emb + "layer_norm.bias").data_ptr(), z.data_ptr(), zst.data_ptr(), xs[0].data_ptr(), xb.data_ptr(),
              rows, 1, H, self.pad, 1e-8, 0.0, seed, 0, s)
-        qb, o = ws.get("bs.q", (rows, H), BF16), ws.get("bs.o", (rows, H), BF16)
-        pr = ws.get("bs.proj", (rows, H), BF16)
-        xbs = [ws.get(f"bs.xb{i}", (rows, H), BF16) for i in (0, 1)]
+        qb, o = ws.get(k + "q", (rows, H), BF16), ws.get(k + "o", (rows, H), BF16)
+        pr = ws.get(k + "proj", (rows, H), BF16)
+        xbs = [ws.get(f"{k}xb{i}", (rows, H), BF16) for i in (0, 1)]
         n = 0
         for l in range(mod.num_layers):
             q = f"textual.transformer.layers.{l}."
@@ -1219,7 +1279,7 @@ class Engine:
                      bias=self.P(q + "multihead_attn.out_proj.bias"))
 
             def ffn(inp, out):
-                self._ffn_fwd(dict(M=rows, H=H, Fd=Fd, p=0.0), dict(q=q, k="bs.", sb=0), inp, out)
+                self._ffn_fwd(dict(M=rows, H=H, Fd=Fd, p=0.0), dict(q=q, k=k, sb=0), inp, out)
 
             for i, run in enumerate((self_attn, cross_attn, ffn), 1):
                 xb = self._residual_sublayer(mod.norm_first, f"{q}norm{i}.", run, xs[n & 1], xb, xs[1 - (n & 1)],
@@ -1249,6 +1309,19 @@ class _BeamState:
     def best(self):
         """int64 (B, L): beam 0 of every image (the best, beams are kept in descending score order)."""
         return self.tokens()[::self.beam].contiguous()
+
+
+class _NucleusState:
+    """Buffers and progress of one running nucleus sampler (Engine.nucleus_start / nucleus_step): L steps have run;
+    pred is the step-major int64 table [max_steps, B] of sampled tokens (row t: token t + 1, SOS is token 0), st.logits
+    the fp32 logits of the last step."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def tokens(self):
+        """int64 (B, L): every caption's tokens so far."""
+        return self.pred[:self.L].t()
 
 
 # ---------------------------------------------------------------------------------------------------- module-level API

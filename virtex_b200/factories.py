@@ -82,11 +82,12 @@ class TextualHeadFactory(Factory):
 
 
 class _DecoderSpec:
-    """Parameters of the reference's beam-search / nucleus-sampling objects.  A captioning model with a `beam_search`
-    decoder captions images by the engine's incremental beam search (CaptioningModel.forward without caption_tokens),
-    which reads its parameters from here; the search itself does not run on this object.  `beam_search` takes the
+    """Parameters of the reference's beam-search / nucleus-sampling objects.  A captioning model captions images
+    (CaptioningModel.forward without caption_tokens) by the engine's incremental beam search for a `beam_search`
+    decoder, or by its incremental nucleus sampler for a `nucleus_sampling` decoder (nucleus_size: the top-p mass), and
+    reads the parameters from here; the decoding itself does not run on this object.  `beam_search` takes the
     reference's per-node beam size of 2, which its factory never overrides (virtex/utils/beam_search.py:40-50,
-    virtex/factories.py:491-500).  Nucleus sampling is not implemented."""
+    virtex/factories.py:491-500)."""
 
     def __init__(self, name, **kwargs):
         self.name = name

@@ -117,6 +117,8 @@ class CaptioningModel(_EngineModel):
         if "caption_tokens" not in batch:
             if self.decoder is None:
                 raise ValueError("Decoder for predicting captions is missing!")
+            if self.decoder.name == "nucleus_sampling":
+                return {"predictions": self._nucleus_sampling(batch["image"])}
             return {"predictions": self._beam_search(batch["image"])}
         image = batch["image"]
         if image.device.type != "cuda":
@@ -154,6 +156,22 @@ class CaptioningModel(_EngineModel):
         with torch.no_grad():
             return self.engine.beam_search(image.contiguous().float(), dec.beam_size, dec.per_node_beam_size,
                                            dec.max_steps, self.sos_index, dec.eos_index)
+
+    def _nucleus_sampling(self, image):
+        """Captions of the forward-direction head by the reference's nucleus sampling (nucleus_sampling.py:47-123),
+        decoded incrementally by the engine: int64 (B, L) on the device.  Each call draws a fresh 64-bit seed on the
+        device from torch's default CUDA generator (no host synchronisation), so torch.manual_seed makes a call
+        reproducible and successive calls sample different captions, as the reference's torch.multinomial does."""
+        dec = self.decoder
+        if self.training:
+            raise RuntimeError("nucleus sampling runs in eval mode (running BatchNorm statistics, no dropout): call "
+                               "model.eval() first")
+        if image.device.type != "cuda":
+            raise NotImplementedError("nucleus sampling runs on the model's CUDA device only; it has no CPU path")
+        with torch.no_grad():
+            seed = torch.empty(1, dtype=torch.int64, device=image.device).random_(-2 ** 63, None)  # all 64 bits
+            return self.engine.nucleus_sample(image.contiguous().float(), dec.nucleus_size, dec.max_steps,
+                                              self.sos_index, dec.eos_index, seed)
 
     def decoding_step(self, visual_features, partial_captions):
         """Logits of the next token of every partial caption (captioning.py:165-213): (B, C, h, w) fp32 features and

@@ -57,6 +57,7 @@ _PROTOS = {
     "vtx_attn_decode": [P, I64, P, P, I64, I64, P, I64, P, I64, I, I, I, I, P],
     "vtx_beam_rows": [P, I64, I, I, P, I, I, P, P, P],
     "vtx_beam_select": [P, P, I, I, I, P, P, P, P, P, P, P, I, I, I, P, P],
+    "vtx_nucleus_sample": [P, I64, I, I, P, I, F, P, I, P, P, P],
     "vtx_image_resample": [P, P, P, P, P, P, I, I, P],
     "vtx_image_gray_sum": [P, P, P, P, I, I, P],
     "vtx_image_jitter_normalize": [P, P, P, P, P, P, I, I, P],
