@@ -350,6 +350,89 @@ int vtx_adamw_step(float* p, const float* g, float* exp_avg, float* exp_avg_sq, 
                    const void* segs, int nseg, const float* ctl, const float* hyper, double beta1, double beta2,
                    float eps, float la_alpha, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * VOC07 linear SVMs (csrc/svm.cu): the per-class LinearSVC(C, class_weight={1: 2, -1: 1}, loss="squared_hinge")
+ * cost sweep with 3-fold cross_val_score(scoring="average_precision") of scripts/clf_voc07.py:56-105 (run once per
+ * class by pool.map, :216-229), with the labels of virtex/data/datasets/downstream.py:151-165.  All P problems
+ * (class, cost, fold-or-full fit) are columns of one truncated-Newton solve of liblinear's L2R_L2LOSS_SVC objective
+ *     f_p(w) = 1/2 |w|^2 + sum_i c_ip max(0, 1 - y_ip w . x~_i)^2,    x~_i = [x_i, 1, 0 ...] (intercept_scaling = 1),
+ * c_ip = 0 on the held-out fold of a cross-validation problem.  Per-problem vectors are fp32 [rows, P] (P % 64 == 0);
+ * the products with X~ are vtx_gemm calls over the split operands written here (x = hi + lo in bf16, the three-term
+ * product hi.hi + hi.lo + lo.hi concatenated along K):
+ *     Z [n_pad, P]  = xcat [n_pad, 3 dp] . op [3 dp, P]          (a_mn 0, b_mn 1),  op = [hi; lo; hi] of W
+ *     G [dp, P]     = xstk [3 n_pad, dp]^T . op [3 n_pad, P]     (a_mn 1, b_mn 1),  op = [hi; lo; hi] of U
+ * Column reductions write partial sums double [k][VTX_SVM_SLICES][P] (k = 1 or 3 quantities) that their consumers
+ * add in a fixed order.  Per-problem state: double scal [VTX_SVM_NSCAL, P] and int32 flags [VTX_SVM_NFLAGS, P], rows
+ * named below; the caller zero-initialises both and W before the first Newton step.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define VTX_SVM_SLICES 32
+#define VTX_SVM_MAX_N 16384 /* samples per problem (line search) and per scored column (average precision) */
+/* scal rows: objective at the start of the Newton step, |grad f|, |grad f(0)|, CG |r|^2, CG tolerance |r|^2, CG beta,
+   line-search step */
+#define VTX_SVM_F 0
+#define VTX_SVM_GNORM 1
+#define VTX_SVM_GNORM0 2
+#define VTX_SVM_RR 3
+#define VTX_SVM_CG_TOL2 4
+#define VTX_SVM_BETA 5
+#define VTX_SVM_STEP 6
+#define VTX_SVM_NSCAL 7
+/* flags rows: status (0 running, 1 converged, 2 Newton-step cap), Newton steps taken, CG done in this step, CG
+   iterations in this step, CG iterations in total, CG iteration cap ever hit */
+#define VTX_SVM_STATUS 0
+#define VTX_SVM_NEWTON 1
+#define VTX_SVM_CG_DONE 2
+#define VTX_SVM_CG_ITERS 3
+#define VTX_SVM_CG_TOTAL 4
+#define VTX_SVM_CG_CAPPED 5
+#define VTX_SVM_NFLAGS 6
+/* x fp32 [n, ldx] (d features) -> x~ = [x, 1, 0 ... 0] with rows n .. n_pad-1 zero, written as xcat bf16 [n_pad, 3 dp]
+   = [hi | hi | lo] and / or xstk bf16 [3 n_pad, dp] = [hi; hi; lo] (either may be NULL); n_pad, dp % 64 == 0, dp > d */
+int vtx_svm_split_x(const float* x, int64_t ldx, int n, int d, int n_pad, int dp, void* xcat, void* xstk, void* stream);
+/* op bf16 [3 rows, P] = [hi; lo; hi] of v fp32 [rows, P] */
+int vtx_svm_split_cols(const float* v, int rows, int P, void* op, void* stream);
+/* From Z and cy = y * c [n, P]: uop = split of u = 2 c (z - y) [y z < 1] (grad f = w + X~^T u), dact = c [y z < 1]
+   (generalised Hessian H = I + 2 X~^T diag(dact) X~), part [1][S][P] = loss sum_i c max(0, 1 - y z)^2 */
+int vtx_svm_margin(const float* z, const float* cy, int n, int P, void* uop, float* dact, double* part, void* stream);
+/* y += x when add; part [3][S][P] = sum y^2, sum x y, sum x^2 (after the add) */
+int vtx_svm_axpy_dot(float* y, const float* x, int rows, int P, int add, double* part, void* stream);
+/* vop = split of 2 dact t */
+int vtx_svm_hess_mid(const float* t, const float* dact, int n, int P, void* vop, void* stream);
+/* One thread per problem, from the margin's loss and the axpy_dot of g += w: objective, |g|, convergence
+   (|g| <= eps |g(0)| -> status 1; max_newton steps taken -> status 2) and the CG set-up (|r|^2 = |g|^2, tolerance
+   0.01 |g|^2: forcing term 0.1); *n_running = problems still running (the one value the host reads per Newton step) */
+int vtx_svm_newton_begin(const double* part_loss, const double* part_g, int P, double* scal, int32_t* flags,
+                         double eps, int max_newton, int32_t* n_running, void* stream);
+/* r = -g, d = r, s = 0 (all zero for problems not running), dop = split of d */
+int vtx_svm_cg_start(const float* g, float* r, float* d, float* s, const int32_t* flags, int rows, int P, void* dop,
+                     void* stream);
+/* CG iteration for problems with CG not done: alpha = rr / (d . Hd) from part_dhd (axpy_dot of Hd = X~^T v + d, row
+   1), s += alpha d, r -= alpha Hd; part_rr [1][S][P] = |r|^2 */
+int vtx_svm_cg_update(float* s, float* r, const float* d, const float* hd, const double* part_dhd, const double* scal,
+                      const int32_t* flags, int rows, int P, double* part_rr, void* stream);
+/* One thread per problem: beta = |r_new|^2 / |r|^2, CG done at |r|^2 <= tolerance or max_cg iterations (CG_CAPPED);
+   *n_running = problems still in CG */
+int vtx_svm_cg_scalars(const double* part_rr, int P, double* scal, int32_t* flags, int max_cg, int32_t* n_running,
+                       void* stream);
+/* d = r + beta d for problems in CG; dop = split of d */
+int vtx_svm_cg_direction(const float* r, float* d, const double* scal, const int32_t* flags, int rows, int P, void* dop,
+                         void* stream);
+/* Exact line search along s, one CTA per running problem, in double: the root of phi'(a) for the convex piecewise
+   quadratic phi(a) = f(w + a s), from z = X~ w, t = X~ s, cy and part_dots (axpy_dot with y = s, x = w: s.s, w.s);
+   writes scal STEP, counts the Newton step, and sets status 1 when phi(0) - phi(step) <= decrease_tol * f.
+   n <= VTX_SVM_MAX_N (z, t, cy staged in shared memory). */
+int vtx_svm_line_search(const float* z, const float* t, const float* cy, int n, int P, const double* part_dots,
+                        double* scal, int32_t* flags, double decrease_tol, void* stream);
+/* w += step s; wop = split of w */
+int vtx_svm_newton_step(float* w, const float* s, const double* scal, int rows, int P, void* wop, void* stream);
+/* sklearn's average_precision_score (sklearn/metrics/_ranking.py: step-wise over distinct thresholds, tied scores one
+   step), one CTA per scored column j: cols int32 [ncols, 3] = (score column, label column, fold).  Sample i < n counts
+   when labels[i * ldl + label column] is 1 (positive) or 0 (negative) and, for fold >= 0, folds[i * ldf + label column]
+   == fold; ap[j] in double, 0 without a positive.  n > VTX_SVM_MAX_N is rejected with VTX_EUNSUPPORTED. */
+int vtx_svm_average_precision(const float* scores, int64_t lds, int n, const int8_t* labels, int64_t ldl,
+                              const int8_t* folds, int64_t ldf, const int32_t* cols, int ncols, double* ap,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

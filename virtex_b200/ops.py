@@ -66,6 +66,19 @@ _PROTOS = {
     "vtx_clip_coef": [P, I, F, P, P],
     "vtx_sgd_step": [P, P, P, P, P, P, I, P, P, F, F, P],
     "vtx_adamw_step": [P, P, P, P, P, P, P, I, P, P, D, D, F, F, P],
+    "vtx_svm_split_x": [P, I64, I, I, I, I, P, P, P],
+    "vtx_svm_split_cols": [P, I, I, P, P],
+    "vtx_svm_margin": [P, P, I, I, P, P, P, P],
+    "vtx_svm_axpy_dot": [P, P, I, I, I, P, P],
+    "vtx_svm_hess_mid": [P, P, I, I, P, P],
+    "vtx_svm_newton_begin": [P, P, I, P, P, D, I, P, P],
+    "vtx_svm_cg_start": [P, P, P, P, P, I, I, P, P],
+    "vtx_svm_cg_update": [P, P, P, P, P, P, P, I, I, P, P],
+    "vtx_svm_cg_scalars": [P, I, P, P, I, P, P],
+    "vtx_svm_cg_direction": [P, P, P, P, I, I, P, P],
+    "vtx_svm_line_search": [P, P, P, I, I, P, P, P, D, P],
+    "vtx_svm_newton_step": [P, P, P, I, I, P, P],
+    "vtx_svm_average_precision": [P, I64, I, P, I64, P, I64, P, I, P, P],
 }
 
 _fn = {}
