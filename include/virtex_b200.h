@@ -433,6 +433,41 @@ int vtx_svm_average_precision(const float* scores, int64_t lds, int n, const int
                               const int8_t* folds, int64_t ldf, const int32_t* cols, int ncols, double* ap,
                               void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Caption metrics (CIDEr) (csrc/cider.cu): cider(predictions, ground_truth, n=4, sigma) of virtex/utils/metrics.py:
+ * 177-264, the score of CocoCaptionsEvaluator.evaluate.  Sentences are int32 word ids in CSR form: words [W] and
+ * sent_off [S + 1].  Image i owns reference sentences img_off[i] .. img_off[i + 1] - 1 and hypothesis sentence i.
+ * Per-occurrence arrays are [W, 4]: entry (w, k - 1) is the k-gram starting at word w (k = 1..4); an entry past its
+ * sentence's end holds gid -1, tf 0, ent -1.
+ * An n-gram's identity is a slot of a device hash table (keys uint64 [capacity], capacity a power of two, zeroed by the
+ * caller): a k-gram is the full key (slot of its (k-1)-gram, last word), so equal slots mean equal n-grams.
+ * Every float reduction runs in a fixed order on one thread: two calls are bit-identical.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define VTX_CIDER_MAX_REFS 32                /* references per image */
+#define VTX_CIDER_MAX_WORDS 256              /* words per sentence */
+#define VTX_CIDER_MAX_IMAGE_WORDS 1024       /* reference words of one image (shared-memory df deduplication) */
+#define VTX_CIDER_MAX_TOTAL_WORDS (1 << 24)  /* reference words, and hypothesis words, of one corpus */
+/* gid [W, 4] = slot of every n-gram, inserted (insert = 1) or looked up (insert = 0: -1 when absent).  The table
+   must have at least twice as many slots as it will hold n-grams. */
+int vtx_cider_intern(const int32_t* words, const int32_t* sent_off, int n_sent, unsigned long long* keys,
+                     int64_t capacity, int insert, int32_t* gid, void* stream);
+/* df [capacity] (zeroed by the caller) += 1 per image for every distinct n-gram of its references, one CTA per image */
+int vtx_cider_df(const int32_t* gid, const int32_t* sent_off, const int32_t* img_off, int n_img, int32_t* df,
+                 void* stream);
+/* One warp per sentence: at the first occurrence of each distinct n-gram (by words) tf = its count in the sentence and
+   ent = tf * (log n_img - log max(1, df[gid])) (df 0 when gid < 0); later occurrences tf 0, ent -1.
+   norm [S, 4] = sqrt(sum of ent^2) per order, summed in position order. */
+int vtx_cider_vectors(const int32_t* words, const int32_t* gid, const int32_t* sent_off, int n_sent, const int32_t* df,
+                      int n_img, int32_t* tf, double* ent, double* norm, void* stream);
+/* img_score [n_img] = 10 * mean_k(sum over references of sim_k) / references, with sim_k of the reference's cider():
+   sum over the hypothesis's distinct k-grams of min(vh, vr) * vr, divided by (|h|_k |r|_k) or 1, times
+   e^(-(len_h - len_r)^2 / (2 sigma^2)), len = max(words - 1, 0).  hyp_off [n_img + 1]; one warp per image. */
+int vtx_cider_score(const int32_t* hyp_gid, const double* hyp_ent, const double* hyp_norm, const int32_t* hyp_off,
+                    const int32_t* ref_gid, const double* ref_ent, const double* ref_norm, const int32_t* ref_off,
+                    const int32_t* img_off, int n_img, double sigma, double* img_score, void* stream);
+/* out[0] = mean of x [n], one CTA in a fixed order */
+int vtx_cider_mean(const double* x, int n, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

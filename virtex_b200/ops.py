@@ -79,6 +79,11 @@ _PROTOS = {
     "vtx_svm_line_search": [P, P, P, I, I, P, P, P, D, P],
     "vtx_svm_newton_step": [P, P, P, I, I, P, P],
     "vtx_svm_average_precision": [P, I64, I, P, I64, P, I64, P, I, P, P],
+    "vtx_cider_intern": [P, P, I, P, I64, I, P, P],
+    "vtx_cider_df": [P, P, P, I, P, P],
+    "vtx_cider_vectors": [P, P, P, I, P, I, P, P, P, P],
+    "vtx_cider_score": [P, P, P, P, P, P, P, P, P, I, D, P, P],
+    "vtx_cider_mean": [P, I, P, P],
 }
 
 _fn = {}
