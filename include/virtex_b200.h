@@ -336,6 +336,75 @@ int vtx_collate_tokens(const int64_t* flat, const int64_t* offs, int64_t* cap, i
                        int T, int max_len, int64_t pad, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * JPEG decoding (csrc/jpeg.cu): compressed baseline / extended-sequential Huffman JPEGs -> uint8 HWC RGB, bit-exact
+ * with cv2.cvtColor(cv2.imdecode(buf, IMREAD_COLOR), COLOR_BGR2RGB), the reference's image reads.  One interleaved
+ * scan, 8-bit, 1 component or YCbCr with luma sampling 1x1 / 2x1 / 1x2 / 2x2 and 1x1 chroma, restart markers optional.
+ * The host parses the headers (virtex_b200/jpeg.py) into, per image n:
+ *   info int32 [B, VTX_JPEG_NI]: the VTX_JPEG_I_* fields; component c at VTX_JPEG_I_COMP + 8c = {h, v, quant table,
+ *     DC table, AC table (indices into quant / huff), blocks per plane row, plane rows of blocks, first block in MCU}
+ *   info64 int64 [B, VTX_JPEG_N64]: the VTX_JPEG_Q_* byte / block offsets
+ *   quant uint16 [*, 64] in natural order;  huff: VTX_JPEG_HUFF_BYTES per table (layout in csrc/jpeg.cu)
+ * Workspaces (sized from the headers by the caller): ent (unstuffed bytes, >= entropy length per image), segments
+ * (seg_start, seg_len, seg_chunk0: VTX_JPEG_I_NSEG per image), chunk slots (VTX_JPEG_I_CHUNK_CAP per image: two
+ * state buffers of int4 and one int32 scan), coef int16 [blocks, 64] (zeroed), planes uint8.  status int32 [B]
+ * (zeroed) collects VTX_JPEG_ST_* bits; rounds int32 [B] (zeroed) the last synchronisation round that changed a chunk.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define VTX_JPEG_NI 48
+#define VTX_JPEG_I_H 0           /* frame height, width */
+#define VTX_JPEG_I_W 1
+#define VTX_JPEG_I_ORIENT 2      /* EXIF orientation 1..8 */
+#define VTX_JPEG_I_NCOMP 3
+#define VTX_JPEG_I_MCUX 4        /* MCUs per row, MCU rows */
+#define VTX_JPEG_I_MCUY 5
+#define VTX_JPEG_I_RI 6          /* restart interval in MCUs, 0 = none */
+#define VTX_JPEG_I_BPM 7         /* blocks per MCU */
+#define VTX_JPEG_I_NSEG 8        /* restart segments = ceil(MCUs / RI), 1 without restarts */
+#define VTX_JPEG_I_SEG_BASE 9    /* first segment slot of the image */
+#define VTX_JPEG_I_CHUNK_BASE 10 /* first chunk slot (ascending over the batch) */
+#define VTX_JPEG_I_CHUNK_CAP 11  /* chunk slots: ceil(entropy bytes * 8 / chunk_bits) + segments */
+#define VTX_JPEG_I_OH 12         /* oriented output height, width */
+#define VTX_JPEG_I_OW 13
+#define VTX_JPEG_I_COMP 16
+#define VTX_JPEG_N64 8
+#define VTX_JPEG_Q_ENT_SRC 0     /* entropy data (after SOS) in src; the EOI marker follows it */
+#define VTX_JPEG_Q_ENT_LEN 1
+#define VTX_JPEG_Q_ENT_DST 2     /* the image's region of ent */
+#define VTX_JPEG_Q_COEF 3        /* first block in coef (ascending over the batch) */
+#define VTX_JPEG_Q_PLANE 4       /* 3 plane offsets in planes */
+#define VTX_JPEG_Q_OUT 7         /* RGB output offset in out */
+#define VTX_JPEG_HUFF_BYTES 1536
+#define VTX_JPEG_ST_MARKER 1     /* unexpected marker, RSTn out of order or restart count mismatch */
+#define VTX_JPEG_ST_BADCODE 2    /* a code missing from the Huffman table */
+#define VTX_JPEG_ST_RUN 4        /* a run past coefficient 63 */
+#define VTX_JPEG_ST_OUT 8        /* a restart segment ran out of bits */
+#define VTX_JPEG_ST_UNSYNCED 16  /* some chunk had not synchronised: run more rounds and decode again */
+/* one CTA per image: strip stuffing, split at RSTn, count chunks of chunk_bits bits per segment */
+int vtx_jpeg_unstuff(const uint8_t* src, const int32_t* info, const int64_t* info64, int B, uint8_t* ent,
+                     int32_t* seg_start, int32_t* seg_len, int32_t* seg_chunk0, int32_t* nchunks, int32_t* status,
+                     int chunk_bits, void* stream);
+/* synchronisation round `round` (0 = speculative decode of every chunk) from st_in into st_out (int4 per slot) */
+int vtx_jpeg_sync(const uint8_t* ent, const int32_t* info, const int64_t* info64, const void* huff,
+                  const int32_t* seg_start, const int32_t* seg_len, const int32_t* seg_chunk0, const int32_t* nchunks,
+                  int B, int slots, const void* st_in, void* st_out, int round, int32_t* rounds, int chunk_bits,
+                  void* stream);
+/* excl [slots] = exclusive scan of the blocks each chunk completes, per image */
+int vtx_jpeg_count_scan(const int32_t* info, const int32_t* nchunks, const void* st, int32_t* excl, int B,
+                        void* stream);
+/* final decode: coefficients (DC as differences) into coef, verification of every chunk's recorded state */
+int vtx_jpeg_coefs(const uint8_t* ent, const int32_t* info, const int64_t* info64, const void* huff,
+                   const int32_t* seg_start, const int32_t* seg_len, const int32_t* seg_chunk0, const int32_t* nchunks,
+                   int B, int slots, const void* st, const int32_t* excl, int16_t* coef, int32_t* status,
+                   int chunk_bits, void* stream);
+/* DC differences -> absolute DC, per component and restart interval */
+int vtx_jpeg_dc_scan(const int32_t* info, const int64_t* info64, int16_t* coef, int B, void* stream);
+/* dequantise + islow IDCT of nblocks blocks into the component planes */
+int vtx_jpeg_idct(const int32_t* info, const int64_t* info64, const int16_t* coef, const uint16_t* quant,
+                  uint8_t* planes, int B, int64_t nblocks, void* stream);
+/* upsampling + YCbCr -> RGB (or grey x 3) + EXIF orientation into out (uint8 HWC RGB at out + info64 Q_OUT) */
+int vtx_jpeg_color(const int32_t* info, const int64_t* info64, const uint8_t* planes, uint8_t* out, int B,
+                   int64_t max_pixels, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Fused optimiser tail over flat fp32 arenas (scripts/pretrain_virtex.py:157-162; virtex/factories.py:529-545;
  * virtex/optim/lookahead.py:82-102).  segs: device array of {int64 begin, int64 end, float lr, float wd}.
  * ctl[0] = gradient scale (clip / world size), ctl[1] = gradient norm; hyper = {lr multiplier, first step, lookahead}.

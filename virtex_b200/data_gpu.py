@@ -3,16 +3,23 @@
 Drop-in for what `CaptioningDataset.__getitem__` + `collate_fn` (virtex/data/datasets/captioning.py:51-100) produce with
 the transform lists of the base config (virtex/factories.py:131-155, `DATA.IMAGE_TRANSFORM_TRAIN/VAL`): the same batch
 dict {"image" fp32 [B,3,224,224], "caption_tokens", "noitpac_tokens", "caption_lengths"}, built on the device from
-decoded uint8 HWC images (any sizes) and token-id lists.  JPEG decoding, tokenisation and the caption-side
-left<->right swap of the paired horizontal flip (virtex/data/transforms.py:29-36, a string operation) stay on the host;
-the host also draws the random parameters, so the kernels are deterministic and testable:
+token-id lists and images of any size, each given either decoded (uint8 HWC RGB array) or encoded (the JPEG file's
+bytes: `bytes`, `bytearray`, `memoryview` or a 1-D uint8 array), mixed freely within a batch.  Encoded images are
+decoded on the device by virtex_b200.jpeg, bit-exact with the reference's cv2.imread + cvtColor(BGR2RGB).
+Tokenisation and the caption-side left<->right swap of the paired horizontal flip (virtex/data/transforms.py:29-36, a
+string operation) stay on the host; the host also draws the random parameters, so the kernels are deterministic and
+testable:
 
     pipe = GpuInputPipeline(device)
-    params = [pipe.sample_train_params(rng, *img.shape[:2]) for img in images]     # or pipe.val_params(H, W)
-    batch = pipe(images, params, token_lists)
+    sizes = [jpeg.image_size(buf) for buf in buffers]                              # or img.shape[:2]
+    params = [pipe.sample_train_params(rng, *hw) for hw in sizes]                  # or pipe.val_params(H, W)
+    batch = pipe(buffers, params, token_lists)
 
-One pinned staging buffer and one H2D copy per batch carry the raw pixels (uint8: 4x fewer PCIe bytes than the fp32
-tensors the reference's DataLoader ships) plus a ~100 B/image parameter table.  No CPU fallback: CUDA tensors out.
+One pinned staging buffer and one H2D copy per batch carry the compressed bytes or raw pixels (uint8: 4x fewer PCIe
+bytes than the fp32 tensors the reference's DataLoader ships) plus a ~100 B/image parameter table.  JPEGs the device
+path does not reproduce (progressive, CMYK, truncated, corrupt entropy data, ...) are decoded by cv2 on the host and
+take the decoded-array path; batch["_jpeg_fallbacks"] (a CPU int64 scalar, present when the batch had encoded images)
+counts them.  No CPU fallback otherwise: CUDA tensors out.
 """
 import math
 from typing import Dict, List, Optional, Sequence
@@ -20,6 +27,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
+from . import jpeg
 from .ops import _stream, call
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
@@ -90,7 +98,19 @@ class GpuInputPipeline:
                  token_lists: Optional[Sequence[Sequence[int]]] = None) -> Dict[str, torch.Tensor]:
         B, S = len(images), self.S
         assert B == len(params) and B > 0
-        arrs = [np.ascontiguousarray(im.cpu().numpy() if torch.is_tensor(im) else im) for im in images]
+        # encoded images: parsed here and decoded on the device, or decoded by cv2 when the device path cannot
+        arrs, heads, blobs = [], {}, {}
+        for n, im in enumerate(images):
+            if jpeg.is_encoded(im):
+                h, b = jpeg.parse_or_none(im)
+                if h is None:
+                    arrs.append(jpeg.host_decode(b, f"image {n}"))
+                else:
+                    arrs.append(None)
+                    heads[n], blobs[n] = h, b
+            else:
+                arrs.append(np.ascontiguousarray(im.cpu().numpy() if torch.is_tensor(im) else im))
+        n_host = sum(jpeg.is_encoded(im) for im in images) - len(heads)
         geom_i = np.zeros((B, 8), np.int32)
         geom_d = np.zeros((B, 2), np.float64)
         jit_i = np.zeros((B, 6), np.int32)
@@ -98,9 +118,12 @@ class GpuInputPipeline:
         offs = np.zeros(B, np.int64)
         total = 0
         for n, (a, p) in enumerate(zip(arrs, params)):
-            if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
-                raise ValueError("images must be uint8 HWC RGB arrays")
-            H, W = a.shape[:2]
+            if a is None:
+                H, W = heads[n].height, heads[n].width
+            elif a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError("images must be uint8 HWC RGB arrays or encoded JPEG bytes")
+            else:
+                H, W = a.shape[:2]
             y0, x0, h, w = p.region
             if not (0 <= y0 and 0 <= x0 and y0 + h <= H and x0 + w <= W and h > 0 and w > 0):
                 raise ValueError(f"crop box {p.region} outside the {H}x{W} image")
@@ -113,26 +136,52 @@ class GpuInputPipeline:
                 jit_i[n, 1] = 1
                 jit_d[n] = p.jitter[:4]
                 jit_i[n, 2:] = p.jitter[4]
-            offs[n] = total
-            total += (a.size + 15) // 16 * 16
+            if a is not None:
+                offs[n] = total
+                total += (a.size + 15) // 16 * 16
+        # compressed bytes follow the pixels; the device decodes them into a region after the staged bytes
+        jidx = sorted(heads)
+        src_off = np.zeros(len(jidx), np.int64)
+        for k, n in enumerate(jidx):
+            src_off[k] = total
+            total += (len(blobs[n]) + 15) // 16 * 16
+        dec_off = np.zeros(len(jidx), np.int64)
+        dec_total = 0
+        for k, n in enumerate(jidx):
+            dec_off[k] = dec_total
+            dec_total += (heads[n].height * heads[n].width * 3 + 15) // 16 * 16
+        plan = jpeg.Plan([heads[n] for n in jidx], src_off, dec_off) if jidx else None
         tok_flat = tok_offs = None
         if token_lists is not None:
             assert len(token_lists) == B
             tok_offs = np.zeros(B + 1, np.int64)
             tok_offs[1:] = np.cumsum([len(t) for t in token_lists])
             tok_flat = np.fromiter((x for t in token_lists for x in t), np.int64, int(tok_offs[-1]))
-        # ---- one pinned staging buffer: [pixels | tables], one H2D copy
+        # decoded JPEG pixels land after the staged bytes (need_al); their offsets are known from the headers
+        tab_bytes0 = sum((t.nbytes + 15) // 16 * 16 for t in [geom_d, jit_d, offs, geom_i, jit_i] +
+                         ([tok_flat, tok_offs] if tok_flat is not None else []) + (plan.tables() if plan else []))
+        need_al = (total + tab_bytes0 + 15) // 16 * 16
+        for k, n in enumerate(jidx):
+            offs[n] = need_al + dec_off[k]
+        # ---- one pinned staging buffer: [pixels | compressed bytes | tables], one H2D copy
         tables = [geom_d, jit_d, offs] + ([tok_flat, tok_offs] if tok_flat is not None else []) + [geom_i, jit_i]
+        if plan is not None:
+            tables += plan.tables()
         tab_bytes = sum((t.nbytes + 15) // 16 * 16 for t in tables)
         need = total + tab_bytes
         if self._pinned is None or self._pinned.numel() < need:
             self._pinned = torch.empty(int(need * 1.25) + 1024, dtype=torch.uint8).pin_memory()
-            self._dev = torch.empty_like(self._pinned, device=self.device)
+        if self._dev is None or self._dev.numel() < need_al + dec_total:
+            self._dev = torch.empty(max(self._pinned.numel(), int((need_al + dec_total) * 1.25)), dtype=torch.uint8,
+                                    device=self.device)
         if self._copied is not None:
             self._copied.synchronize()  # the previous batch's copy must have left the staging buffer
         host = self._pinned.numpy()
         for a, o in zip(arrs, offs):
-            host[o:o + a.size] = a.reshape(-1)
+            if a is not None:
+                host[o:o + a.size] = a.reshape(-1)
+        for k, n in enumerate(jidx):
+            host[src_off[k]:src_off[k] + len(blobs[n])] = np.frombuffer(blobs[n], np.uint8)
         views, cur = [], total
         for t in tables:
             host[cur:cur + t.nbytes] = np.frombuffer(t.tobytes(), np.uint8)
@@ -144,6 +193,16 @@ class GpuInputPipeline:
         base = self._dev.data_ptr()
         ptr = {id(t): base + o for o, t in views}
         s = _stream()
+        if plan is not None:
+            status = jpeg.decoder_for(self.device).run(plan, base, [ptr[id(t)] for t in plan.tables()], base + need_al)
+            for k, n in enumerate(jidx):
+                if status[k]:  # the device found the entropy data corrupt: cv2 decodes it (what the reference reads)
+                    a = jpeg.host_decode(blobs[n], f"image {n}")
+                    if a.shape[:2] != (heads[n].height, heads[n].width):
+                        raise ValueError(f"image {n}: cv2 decoded {a.shape[:2]}, the headers say "
+                                         f"{(heads[n].height, heads[n].width)}")
+                    self._dev[offs[n]:offs[n] + a.size].copy_(torch.from_numpy(a.reshape(-1)))
+                    n_host += 1
         img_u8 = torch.empty(B, S, S, 3, dtype=torch.uint8, device=self.device)
         gray = torch.zeros(B, dtype=torch.int64, device=self.device)
         out = torch.empty(B, 3, S, S, dtype=torch.float32, device=self.device)
@@ -153,6 +212,8 @@ class GpuInputPipeline:
         call("vtx_image_jitter_normalize", img_u8.data_ptr(), ptr[id(jit_i)], ptr[id(jit_d)], gray.data_ptr(),
              self.norm.data_ptr(), out.data_ptr(), B, S, s)
         batch = {"image": out, "_image_u8": img_u8}
+        if any(jpeg.is_encoded(im) for im in images):
+            batch["_jpeg_fallbacks"] = torch.tensor(n_host, dtype=torch.int64)
         if tok_flat is not None:
             T = int(min(self.max_len, max(len(t) for t in token_lists)))
             cap = torch.empty(B, T, dtype=torch.int64, device=self.device)

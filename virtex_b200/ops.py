@@ -62,6 +62,13 @@ _PROTOS = {
     "vtx_image_gray_sum": [P, P, P, P, I, I, P],
     "vtx_image_jitter_normalize": [P, P, P, P, P, P, I, I, P],
     "vtx_collate_tokens": [P, P, P, P, P, I, I, I, I64, P],
+    "vtx_jpeg_unstuff": [P, P, P, I, P, P, P, P, P, P, I, P],
+    "vtx_jpeg_sync": [P, P, P, P, P, P, P, P, I, I, P, P, I, P, I, P],
+    "vtx_jpeg_count_scan": [P, P, P, P, I, P],
+    "vtx_jpeg_coefs": [P, P, P, P, P, P, P, P, I, I, P, P, P, P, I, P],
+    "vtx_jpeg_dc_scan": [P, P, P, I, P],
+    "vtx_jpeg_idct": [P, P, P, P, P, I, I64, P],
+    "vtx_jpeg_color": [P, P, P, P, I, I64, P],
     "vtx_sumsq": [P, I64, P, P],
     "vtx_clip_coef": [P, I, F, P, P],
     "vtx_sgd_step": [P, P, P, P, P, P, I, P, P, F, F, P],
