@@ -30,6 +30,13 @@ Comparisons treat +0 and -0 as equal: the kernels' fmaxf(v, 0) may keep either s
 import torch
 
 F32, F64 = torch.float32, torch.float64
+U = 2.0 ** -24  # unit roundoff of fp32
+
+
+def ulp_bf16(x):
+    """Spacing of bf16 numbers at |x| (the smallest normal spacing below 2^-126)."""
+    e = torch.floor(torch.log2(x.abs())).clamp_min(-126)
+    return torch.exp2(e - 7)
 
 
 def f32(x):
@@ -144,3 +151,36 @@ def bn_scale_shift(gamma, beta, mean, invstd):
     """Rows 2 and 3 of bnp from the device's own invstd: scale = gamma * invstd, shift = fma(scale, -mean, beta)."""
     sc = f32(gamma * invstd)
     return sc, fma_f32(sc, -mean, beta)
+
+
+def reduce_depth(sms, M, C, two):
+    """Sequential depth of vtx_bn_bwd_reduce's fp32 accumulation (mirrors its launch geometry): terms per thread + rows
+    reduced per CTA + atomics per channel."""
+    rows_par = 256 // (C // 8)
+    ku = 4 if two else 5
+    blocks = min(-(-M // (rows_par * ku)), sms * (1 if two else 2))
+    return -(-M // (rows_par * blocks)) + rows_par + blocks
+
+
+def bn_bwd_sums(dz, y, bnp, depth):
+    """BN-backward sums [sum_m dz, sum_m dz * (y - mean) * invstd] of [M, C] dz (float64) and bf16 y with the device's
+    fp32 bnp, in float64, and their bound (depth + 3) * 2^-24 * sum |term| for an fp32 accumulation of sequential depth
+    `depth` (the 3 for the rounding of each term).  dgamma += sums[1], dbeta += sums[0]."""
+    t = dz * (y.to(F64) - bnp[0].to(F64)) * bnp[1].to(F64)
+    ref = torch.stack([dz.sum(0), t.sum(0)])
+    tol = (depth + 3) * U * torch.stack([dz.abs().sum(0), t.abs().sum(0)]) + 1e-30
+    return ref, tol
+
+
+def bn_bwd_dy(dz, y, bnp, sums, M):
+    """Train-mode BN backward dy = k0 * dz + k1 * y + k2 of [M, C] dz (float64) and y with the device's bnp and sums
+    (k0 = scale, k1 = -scale * m2 * invstd, k2 = scale * (m2 * invstd * mean - m1), m1 / m2 = sums / M), and its
+    bound: 1 bf16 ulp plus 2^-21 * (|k0 dz| + |k1 y| + |scale| * (|m2 invstd mean| + |m1|)) for the fp32 coefficients
+    (k2 cancels when |mean| is large) and their evaluation."""
+    yd = y.to(F64)
+    scl, mean, istd = bnp[2].to(F64), bnp[0].to(F64), bnp[1].to(F64)
+    m1, m2 = sums[0].to(F64) / M, sums[1].to(F64) / M
+    k0, k1, k2 = scl, -scl * m2 * istd, scl * (m2 * istd * mean - m1)
+    ref = k0 * dz + k1 * yd + k2
+    floor = 2.0 ** -21 * ((k0 * dz).abs() + (k1 * yd).abs() + scl.abs() * ((m2 * istd * mean).abs() + m1.abs()))
+    return ref, ulp_bf16(ref) + floor

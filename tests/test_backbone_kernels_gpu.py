@@ -39,7 +39,7 @@ pytestmark = pytest.mark.gpu
 
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 DEV = "cuda"
-U = 2.0 ** -24
+U = R.U
 MOM, EPS = 0.1, 1e-5
 EXTRA = 3  # rows beyond M that must stay untouched
 WIDTHS = (64, 128, 256, 512, 1024, 2048)
@@ -78,11 +78,6 @@ def _d(t):
 def ulp_f32(x):
     e = torch.floor(torch.log2(x.abs())).clamp_min(-126)
     return torch.exp2(e - 23)
-
-
-def ulp_bf16(x):
-    e = torch.floor(torch.log2(x.abs())).clamp_min(-126)
-    return torch.exp2(e - 7)
 
 
 def assert_equal(got, want, what):
@@ -257,29 +252,13 @@ def test_bn_act_and_fused_finalize_act(C, M):
 
 # ------------------------------------------------------------------------------------------------ BN backward
 def _reduce_depth(ops, M, C, two):
-    """Sequential depth of vtx_bn_bwd_reduce's fp32 accumulation (mirrors its launch geometry)."""
-    rows_par = 256 // (C // 8)
-    ku = 4 if two else 5
-    blocks = min(-(-M // (rows_par * ku)), ops.num_sms() * (1 if two else 2))
-    return -(-M // (rows_par * blocks)) + rows_par + blocks
+    return R.reduce_depth(ops.num_sms(), M, C, two)
 
 
 def _check_sums(sums, dz, y, bnp, depth, what):
-    t = dz * (_d(y) - _d(bnp[0])) * _d(bnp[1])
-    for row, terms in ((0, dz), (1, t)):
-        ref = terms.sum(0)
-        tol = (depth + 3) * U * terms.abs().sum(0) + 1e-30
-        assert_within(sums[row], ref, tol, f"{what}: sums[{row}]")
-
-
-def _dy_reference(dz, y, bnp, sums, M):
-    yd = _d(y)
-    scl, mean, istd = _d(bnp[2]), _d(bnp[0]), _d(bnp[1])
-    m1, m2 = _d(sums[0]) / M, _d(sums[1]) / M
-    k0, k1, k2 = scl, -scl * m2 * istd, scl * (m2 * istd * mean - m1)
-    ref = k0 * dz + k1 * yd + k2
-    floor = 2.0 ** -21 * ((k0 * dz).abs() + (k1 * yd).abs() + scl.abs() * ((m2 * istd * mean).abs() + m1.abs()))
-    return ref, ulp_bf16(ref) + floor
+    ref, tol = R.bn_bwd_sums(dz, y, bnp, depth)
+    for row in range(2):
+        assert_within(sums[row], ref[row], tol[row], f"{what}: sums[{row}]")
 
 
 def _bwd_setup(ops, C, M, g):
@@ -354,7 +333,7 @@ def test_bn_backward_reduce_finalize_apply(C, M):
             res[path, with_dz] = (dy, dy2, dzo)
         dy, dy2, dzo = res["unfused", True]
         assert_equal(dzo[:M], dz, what + ": dz_out")
-        refs = [_dy_reference(dz, y[:M], bnp, sums, M)] + ([_dy_reference(dz, y2[:M], bnp2, sums2, M)] if two else [])
+        refs = [R.bn_bwd_dy(dz, y[:M], bnp, sums, M)] + ([R.bn_bwd_dy(dz, y2[:M], bnp2, sums2, M)] if two else [])
         for key, (d1, d2, dz_o) in res.items():
             for k, (got, base) in enumerate(((d1, dy), (d2, dy2))[:len(refs)]):
                 ref, tol = refs[k]
@@ -363,7 +342,7 @@ def test_bn_backward_reduce_finalize_apply(C, M):
                 if key[0] == "unfused":
                     assert torch.equal(got.view(torch.int16), base.view(torch.int16)), f"{what} {key}: dy{k + 1}"
                 else:
-                    assert_within(got[:M], _d(base[:M]), tol + ulp_bf16(_d(base[:M])),
+                    assert_within(got[:M], _d(base[:M]), tol + R.ulp_bf16(_d(base[:M])),
                                   f"{what} {key}: dy{k + 1} vs unfused")
                 assert bool((got[M:] == -3.0).all()), f"{what} {key}: dy{k + 1} rows beyond M written"
             if dz_o is not None:
@@ -593,7 +572,7 @@ def test_nhwc_to_nchw_f32(N, HW, C):
     assert bool((out[N * C * HW:] == -3.0).all())
 
 
-@pytest.mark.parametrize("H,W", [(224, 224), (200, 200), (199, 200)])
+@pytest.mark.parametrize("H,W", [(224, 224), (200, 200), (199, 200), (199, 230), (7, 9)])
 def test_stem_im2col_matches_unfold(H, W):
     _need_cuda()
     ops = _ops()

@@ -32,13 +32,14 @@ static inline int row_threads(int cg, int extent) {
 // ---------------------------------------------------------------------------------------------- stem im2col
 // image fp32 NCHW [N,3,H,W] -> cols bf16 [N*Ho*Wo, ldc], k = (kh*7 + kw)*3 + c for the 7x7/stride 2/pad 3 stem,
 // columns [147, ldc) zero.  One CTA per output row (n, ho): the 7 x 3 input rows it needs are staged in shared memory
-// with coalesced float4 loads, then the ldc-wide column rows are written as coalesced 16-byte vectors.
+// with coalesced float4 loads (scalar loads when W % 4 != 0, where image rows are not 16-byte aligned), then the
+// ldc-wide column rows are written as coalesced 16-byte vectors.
 __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restrict__ img, __nv_bfloat16* __restrict__ cols,
                                                          int N, int H, int W, int Ho, int Wo, int ldc) {
   VTX_PDL_TRIGGER();
-  extern __shared__ float tile[];  // [3][7][Wp], Wp = W + 8: 4 zero columns on each side (left pad 3 -> x offset 4)
-  __shared__ int lut[160];         // k -> (c*7 + kh)*Wp + kw  or -1
-  const int Wp = W + 8;
+  extern __shared__ float tile[];  // [3][7][Wp], Wp = W + 8 rounded up to 4: at least 4 zero columns on each side
+  __shared__ int lut[160];         // k -> (c*7 + kh)*Wp + kw  or -1   (left pad 3 -> x offset 4)
+  const int Wp = (W + 8 + 3) / 4 * 4;
   const int n = blockIdx.x / Ho, ho = blockIdx.x % Ho;
   for (int k = threadIdx.x; k < 160; k += blockDim.x) {
     int v = -1;
@@ -49,16 +50,25 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restric
     lut[k] = v;
   }
   // stage rows: tile[c][r][4 + w] = img[n][c][2*ho - 3 + r][w]
-  const int quads = Wp / 4;
-  for (int e = threadIdx.x; e < 21 * quads; e += blockDim.x) {
-    const int cr = e / quads, qd = e % quads;
-    const int c = cr / 7, r = cr % 7;
-    const int h = 2 * ho - 3 + r;
-    const int w0 = qd * 4 - 4;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (h >= 0 && h < H && w0 >= 0 && w0 + 3 < W)
-      v = *reinterpret_cast<const float4*>(img + (((long long)n * 3 + c) * H + h) * W + w0);
-    *reinterpret_cast<float4*>(tile + cr * Wp + qd * 4) = v;
+  if (W % 4 == 0) {
+    const int quads = Wp / 4;
+    for (int e = threadIdx.x; e < 21 * quads; e += blockDim.x) {
+      const int cr = e / quads, qd = e % quads;
+      const int c = cr / 7, r = cr % 7;
+      const int h = 2 * ho - 3 + r;
+      const int w0 = qd * 4 - 4;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (h >= 0 && h < H && w0 >= 0 && w0 + 3 < W)
+        v = *reinterpret_cast<const float4*>(img + (((long long)n * 3 + c) * H + h) * W + w0);
+      *reinterpret_cast<float4*>(tile + cr * Wp + qd * 4) = v;
+    }
+  } else {
+    for (int e = threadIdx.x; e < 21 * Wp; e += blockDim.x) {
+      const int cr = e / Wp, x = e % Wp;
+      const int c = cr / 7, r = cr % 7;
+      const int h = 2 * ho - 3 + r, w = x - 4;
+      tile[e] = (h >= 0 && h < H && w >= 0 && w < W) ? img[(((long long)n * 3 + c) * H + h) * W + w] : 0.f;
+    }
   }
   __syncthreads();
   const int groups = ldc / 8;
@@ -1052,9 +1062,9 @@ static const char kBnGroupMsg[] = "needs 256 % (C / 8) == 0, i.e. C in {8, 16, 3
 
 extern "C" int vtx_stem_im2col(const float* img, void* cols, int N, int H, int W, int ldc, void* stream) {
   REQ(img && cols && ldc >= 152 && ldc % 8 == 0, "bad arguments");
-  REQ(W % 4 == 0 && ldc <= 160 + 96, "stem im2col needs W %% 4 == 0");
+  REQ(ldc <= 160 + 96, "bad arguments");
   const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-  const size_t smem = (size_t)21 * (W + 8) * sizeof(float);
+  const size_t smem = (size_t)21 * ((W + 8 + 3) / 4 * 4) * sizeof(float);
   REQ(smem <= 48 * 1024, "image too wide for the stem im2col tile");
   stem_im2col_kernel<<<N * Ho, 256, smem, STREAM>>>(img, (__nv_bfloat16*)cols, N, H, W, Ho, Wo, ldc);
   return check_launch("stem_im2col");
