@@ -133,9 +133,10 @@ class Engine:
 
     # BN-backward reductions (sum dz, sum dz * xhat) are accumulated by the epilogue of the GEMM that produces the
     # gradient (bn1 / bn2 of every block, bn3 of blocks followed by an identity block) instead of a separate pass.
-    # bn3's only for the large early-layer tensors: at layer3 / layer4 sizes the longer epilogue costs about what the
-    # stand-alone pass costs.
-    fuse_bn3_min_rows = 100000
+    # bn3's for layer1-3 at batch 256 (the streaming masked-residual dgrad kernel of csrc/gemm_resid.cu reads y and the
+    # mask beside dOut at HBM rate); layer4 and small batches keep the stand-alone pass, which costs about what the
+    # persistent kernel's longer epilogue does.
+    fuse_bn3_min_rows = 40000
 
     def __init__(self, visual=None, textual=None, backward_textual=None, prefix_map=None, ignore_indices=None):
         self.visual, self.textual, self.backward_textual = visual, textual, backward_textual
