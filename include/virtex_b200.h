@@ -334,6 +334,18 @@ int vtx_image_jitter_normalize(const uint8_t* img, const int32_t* jit_i, const d
 /* flat token ids + offsets [B+1] -> caption / reversed caption [B, T] right-padded with pad, lengths [B] (<= max_len) */
 int vtx_collate_tokens(const int64_t* flat, const int64_t* offs, int64_t* cap, int64_t* rev, int64_t* lengths, int B,
                        int T, int max_len, int64_t pad, void* stream);
+/* The masked-LM collate (MaskedLmDataset.__getitem__ + collate_fn, virtex/data/datasets/masked_lm.py:64-119): the
+   trim + right-pad of vtx_collate_tokens into cap, then, per caption of trimmed length n, k = ceil((n - 2) * proportion)
+   (float64) distinct positions of 1 .. n-2 -- the k smallest (key, position), key = hash_u64(*seed, 5000, ctr) -- each
+   turned into mask_id with labels = the original id when k == 1 or u <= mask_prob, into the id
+   mulhi(hash_u64(*seed, 5002, ctr), vocab) of [0, vocab) when u <= mask_prob + replace_prob (float64 sum), and left
+   as it is otherwise; u = (hash_u64(*seed, 5001, ctr) >> 11) * 2^-53, ctr = caption << 32 | position.  labels [B, T]
+   holds pad everywhere else.  The seed is read on the device.  T <= VTX_MLM_MAX_T (one CTA per caption); proportion,
+   mask_prob and replace_prob in [0, 1]; vocab > 0. */
+#define VTX_MLM_MAX_T 1024
+int vtx_collate_masked_lm(const int64_t* flat, const int64_t* offs, int64_t* cap, int64_t* labels, int64_t* lengths,
+                          int B, int T, int max_len, int64_t pad, int64_t mask_id, int64_t vocab, double proportion,
+                          double mask_prob, double replace_prob, const uint64_t* seed, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * JPEG decoding (csrc/jpeg.cu): compressed baseline / extended-sequential Huffman JPEGs -> uint8 HWC RGB, bit-exact

@@ -220,6 +220,59 @@ __global__ void collate_tokens_kernel(const long long* __restrict__ flat, const 
   if (t == 0) lengths[b] = len;
 }
 
+// The masked-LM collate: vtx_collate_tokens' trim + right-pad, then virtex/data/datasets/masked_lm.py:64-91's masking
+// of every caption.  One CTA per caption, one thread per position; a caption of trimmed length n picks
+// k = ceil((n - 2) * proportion) of its positions 1 .. n-2: the k smallest (key, position) pairs, each key an
+// independent 64-bit hash, so every k-subset is equally likely (random.sample's distribution).  A picked position
+// becomes [MASK] (label = the original id) when k == 1 or its uniform u <= mask_prob, a uniform id of [0, vocab) (no
+// label) when u <= mask_prob + replace_prob, and stays as it is (no label) otherwise.  All draws are hash_u64 of
+// (seed, site, caption << 32 | position): the host replays them bit for bit (tests/masked_lm_oracle.py).
+constexpr uint32_t kMlmKeySite = 5000u, kMlmFlagSite = 5001u, kMlmTokenSite = 5002u;  // dropout < 2000, nucleus 4000
+
+__global__ void __launch_bounds__(VTX_MLM_MAX_T) collate_masked_lm_kernel(
+    const long long* __restrict__ flat, const long long* __restrict__ offs, long long* __restrict__ cap,
+    long long* __restrict__ labels, long long* __restrict__ lengths, int T, int max_len, long long pad, long long mask_id,
+    long long vocab, double proportion, double mask_prob, double replace_prob, const uint64_t* __restrict__ seed_ptr) {
+  VTX_PDL_TRIGGER();
+  __shared__ uint64_t keys[VTX_MLM_MAX_T];
+  const int b = blockIdx.x, t = threadIdx.x;
+  const long long o = offs[b];
+  const int n = (int)min((long long)max_len, offs[b + 1] - o);
+  const uint64_t seed = *seed_ptr;
+  const uint64_t ctr = ((uint64_t)b << 32) | (uint32_t)t;
+  const bool cand = t >= 1 && t < n - 1;
+  if (t < T) keys[t] = cand ? hash_u64(seed, kMlmKeySite, ctr) : 0ull;
+  __syncthreads();
+  if (t >= T) return;
+  long long tok = t < n ? flat[o + t] : pad, lab = pad;
+  if (cand) {
+    const int k = (int)ceil(__dmul_rn((double)(n - 2), proportion));  // Python's math.ceil((n - 2) * p), p <= 1
+    const uint64_t mine = keys[t];
+    int rank = 0;
+    for (int q = 1; q < n - 1; ++q) {
+      const uint64_t kq = keys[q];
+      rank += (kq < mine) || (kq == mine && q < t);
+    }
+    if (rank < k) {
+      bool mask = k == 1;
+      if (!mask) {
+        const double u = (double)(hash_u64(seed, kMlmFlagSite, ctr) >> 11) * 0x1p-53;
+        if (u <= mask_prob)
+          mask = true;
+        else if (u <= __dadd_rn(mask_prob, replace_prob))
+          tok = (long long)__umul64hi(hash_u64(seed, kMlmTokenSite, ctr), (uint64_t)vocab);
+      }
+      if (mask) {
+        lab = tok;
+        tok = mask_id;
+      }
+    }
+  }
+  cap[(long long)b * T + t] = tok;
+  labels[(long long)b * T + t] = lab;
+  if (t == 0) lengths[b] = n;
+}
+
 }  // namespace vtx
 
 using namespace vtx;
@@ -256,4 +309,20 @@ extern "C" int vtx_collate_tokens(const int64_t* flat, const int64_t* offs, int6
                                                                  (long long*)cap, (long long*)rev, (long long*)lengths, B,
                                                                  T, max_len, (long long)pad);
   return check_launch("collate_tokens");
+}
+extern "C" int vtx_collate_masked_lm(const int64_t* flat, const int64_t* offs, int64_t* cap, int64_t* labels,
+                                     int64_t* lengths, int B, int T, int max_len, int64_t pad, int64_t mask_id,
+                                     int64_t vocab, double proportion, double mask_prob, double replace_prob,
+                                     const uint64_t* seed, void* stream) {
+  const auto prob = [](double p) { return p >= 0.0 && p <= 1.0; };  // false for NaN
+  if (!flat || !offs || !cap || !labels || !lengths || !seed || B <= 0 || T <= 0 || T > VTX_MLM_MAX_T || vocab <= 0 ||
+      !prob(proportion) || !prob(mask_prob) || !prob(replace_prob))
+    return set_error(VTX_EINVAL, "vtx_collate_masked_lm: bad arguments (T <= %d, probabilities in [0, 1], vocab > 0)",
+                     VTX_MLM_MAX_T);
+  const int threads = (T + 31) / 32 * 32;
+  collate_masked_lm_kernel<<<B, threads, 0, STREAM>>>((const long long*)flat, (const long long*)offs, (long long*)cap,
+                                                      (long long*)labels, (long long*)lengths, T, max_len,
+                                                      (long long)pad, (long long)mask_id, (long long)vocab, proportion,
+                                                      mask_prob, replace_prob, seed);
+  return check_launch("collate_masked_lm");
 }

@@ -20,6 +20,9 @@ bytes than the fp32 tensors the reference's DataLoader ships) plus a ~100 B/imag
 path does not reproduce (progressive, CMYK, truncated, corrupt entropy data, ...) are decoded by cv2 on the host and
 take the decoded-array path; batch["_jpeg_fallbacks"] (a CPU int64 scalar, present when the batch had encoded images)
 counts them.  No CPU fallback otherwise: CUDA tensors out.
+
+The same call builds the batches of the other pretext tasks (`task`, below): masked language modelling, with the
+reference's token masking drawn on the device, and token / multilabel classification.
 """
 import math
 from typing import Dict, List, Optional, Sequence
@@ -42,19 +45,54 @@ class ImageParams:
         self.region, self.resized, self.offset, self.flip, self.jitter = region, resized, offset, flip, jitter
 
 
+TASKS = ("captioning", "masked_lm", "token_classification", "multilabel_classification")
+# MODEL.NAME -> the batch a model of that name trains on
+_TASK_OF_MODEL = {"virtex": "captioning", "bicaptioning": "captioning", "captioning": "captioning",
+                  "masked_lm": "masked_lm", "token_classification": "token_classification",
+                  "multilabel_classification": "multilabel_classification"}
+
+
 class GpuInputPipeline:
+    """`task` chooses the batch built from `token_lists` (captioning by default, as above):
+
+      masked_lm                  "caption_tokens" (masked), "masked_labels", "caption_lengths": MaskedLmDataset's
+                                 masking and collate (virtex/data/datasets/masked_lm.py:64-119), padded with
+                                 `padding_idx`, drawn on the device (vtx_collate_masked_lm)
+      token_classification       "labels": the trimmed token lists padded with `padding_idx` (TokenClassificationDataset)
+      multilabel_classification  "labels": `token_lists` are the per-image category lists, padded with 0 and never
+                                 trimmed (MultiLabelClassificationDataset)
+
+    `GpuInputPipeline.from_config(config, device)` takes every setting from a Config."""
+
     def __init__(self, device, crop_size: int = 224, max_caption_length: int = 30, padding_idx: int = 0,
-                 mean=IMAGENET_MEAN, std=IMAGENET_STD):
+                 mean=IMAGENET_MEAN, std=IMAGENET_STD, task: str = "captioning", vocab_size: int = 10000,
+                 mask_index: int = 3, mask_proportion: float = 0.15, mask_probability: float = 0.85,
+                 replace_probability: float = 0.10):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("GpuInputPipeline runs on a CUDA device (there is no CPU path)")
+        if task not in TASKS:
+            raise ValueError(f"task {task!r} is not one of {TASKS}")
         self.S, self.max_len, self.pad = crop_size, max_caption_length, padding_idx
+        self.task, self.vocab_size, self.mask_index = task, vocab_size, mask_index
+        self.mask_proportion, self.mask_probability = mask_proportion, mask_probability
+        self.replace_probability = replace_probability
         m = np.array(mean, np.float32) * np.float32(255.0)
         inv = np.float32(1) / (np.array(std, np.float32) * np.float32(255.0))
         self.norm = torch.from_numpy(np.concatenate([m, inv])).to(self.device)
         self._pinned: Optional[torch.Tensor] = None
         self._dev: Optional[torch.Tensor] = None
         self._copied: Optional[torch.cuda.Event] = None  # the last H2D copy out of the pinned staging buffer
+
+    @classmethod
+    def from_config(cls, config, device) -> "GpuInputPipeline":
+        """The pipeline of `config`'s MODEL.NAME with DATA.IMAGE_CROP_SIZE, MAX_CAPTION_LENGTH, UNK_INDEX (padding),
+        VOCAB_SIZE, MASK_INDEX and MASKED_LM.* (virtex/factories.py:230-243)."""
+        D = config.DATA
+        return cls(device, crop_size=D.IMAGE_CROP_SIZE, max_caption_length=D.MAX_CAPTION_LENGTH,
+                   padding_idx=D.UNK_INDEX, task=_TASK_OF_MODEL[config.MODEL.NAME], vocab_size=D.VOCAB_SIZE,
+                   mask_index=D.MASK_INDEX, mask_proportion=D.MASKED_LM.MASK_PROPORTION,
+                   mask_probability=D.MASKED_LM.MASK_PROBABILITY, replace_probability=D.MASKED_LM.REPLACE_PROBABILITY)
 
     # ------------------------------------------------------------------------------------------- host-side sampling
     def sample_train_params(self, rng: np.random.Generator, H: int, W: int, scale=(0.2, 1.0), ratio=(0.75, 1.333),
@@ -95,7 +133,11 @@ class GpuInputPipeline:
 
     # ------------------------------------------------------------------------------------------------------- batch
     def __call__(self, images: Sequence, params: Sequence[ImageParams],
-                 token_lists: Optional[Sequence[Sequence[int]]] = None) -> Dict[str, torch.Tensor]:
+                 token_lists: Optional[Sequence[Sequence[int]]] = None,
+                 seed: Optional[int] = None) -> Dict[str, torch.Tensor]:
+        """The batch of `images` (with `params`) and `token_lists` for the pipeline's task.  masked_lm draws its 64-bit
+        seed on the device from torch's default CUDA generator (no host synchronisation: torch.manual_seed reproduces
+        a batch, successive batches differ), or takes `seed` when given."""
         B, S = len(images), self.S
         assert B == len(params) and B > 0
         # encoded images: parsed here and decoded on the device, or decoded by cv2 when the device path cannot
@@ -157,14 +199,19 @@ class GpuInputPipeline:
             tok_offs = np.zeros(B + 1, np.int64)
             tok_offs[1:] = np.cumsum([len(t) for t in token_lists])
             tok_flat = np.fromiter((x for t in token_lists for x in t), np.int64, int(tok_offs[-1]))
+        tok_tabs = [tok_flat, tok_offs] if tok_flat is not None else []
+        seed_tab = None
+        if tok_flat is not None and self.task == "masked_lm" and seed is not None:
+            seed_tab = np.array([int(seed) & (2 ** 64 - 1)], np.uint64)  # travels with the batch's one copy
+            tok_tabs.append(seed_tab)
         # decoded JPEG pixels land after the staged bytes (need_al); their offsets are known from the headers
-        tab_bytes0 = sum((t.nbytes + 15) // 16 * 16 for t in [geom_d, jit_d, offs, geom_i, jit_i] +
-                         ([tok_flat, tok_offs] if tok_flat is not None else []) + (plan.tables() if plan else []))
+        tab_bytes0 = sum((t.nbytes + 15) // 16 * 16 for t in [geom_d, jit_d, offs, geom_i, jit_i] + tok_tabs +
+                         (plan.tables() if plan else []))
         need_al = (total + tab_bytes0 + 15) // 16 * 16
         for k, n in enumerate(jidx):
             offs[n] = need_al + dec_off[k]
         # ---- one pinned staging buffer: [pixels | compressed bytes | tables], one H2D copy
-        tables = [geom_d, jit_d, offs] + ([tok_flat, tok_offs] if tok_flat is not None else []) + [geom_i, jit_i]
+        tables = [geom_d, jit_d, offs] + tok_tabs + [geom_i, jit_i]
         if plan is not None:
             tables += plan.tables()
         tab_bytes = sum((t.nbytes + 15) // 16 * 16 for t in tables)
@@ -215,11 +262,29 @@ class GpuInputPipeline:
         if any(jpeg.is_encoded(im) for im in images):
             batch["_jpeg_fallbacks"] = torch.tensor(n_host, dtype=torch.int64)
         if tok_flat is not None:
-            T = int(min(self.max_len, max(len(t) for t in token_lists)))
-            cap = torch.empty(B, T, dtype=torch.int64, device=self.device)
-            rev = torch.empty(B, T, dtype=torch.int64, device=self.device)
-            lens = torch.empty(B, dtype=torch.int64, device=self.device)
-            call("vtx_collate_tokens", ptr[id(tok_flat)], ptr[id(tok_offs)], cap.data_ptr(), rev.data_ptr(),
-                 lens.data_ptr(), B, T, self.max_len, self.pad, s)
-            batch.update(caption_tokens=cap, noitpac_tokens=rev, caption_lengths=lens)
+            batch.update(self._collate(B, token_lists, ptr[id(tok_flat)], ptr[id(tok_offs)],
+                                       ptr[id(seed_tab)] if seed_tab is not None else None, s))
         return batch
+
+    def _collate(self, B, token_lists, flat, offs, seed_ptr, s) -> Dict[str, torch.Tensor]:
+        """The task's token / label tensors from the staged flat lists (device pointers)."""
+        longest = max(len(t) for t in token_lists)
+        # category lists are not captions: no trimming, padding with 0 (MultiLabelClassificationDataset.collate_fn)
+        max_len, pad = (longest, 0) if self.task == "multilabel_classification" else (self.max_len, self.pad)
+        T = int(min(max_len, longest))
+        new = lambda *shape: torch.empty(*shape, dtype=torch.int64, device=self.device)
+        cap, lens = new(B, T), new(B)
+        if self.task == "masked_lm":
+            labels = new(B, T)
+            if seed_ptr is None:
+                seed_t = new(1).random_(-2 ** 63, None)  # all 64 bits, from torch's default CUDA generator
+                seed_ptr = seed_t.data_ptr()
+            call("vtx_collate_masked_lm", flat, offs, cap.data_ptr(), labels.data_ptr(), lens.data_ptr(), B, T, max_len,
+                 pad, self.mask_index, self.vocab_size, self.mask_proportion, self.mask_probability,
+                 self.replace_probability, seed_ptr, s)
+            return {"caption_tokens": cap, "masked_labels": labels, "caption_lengths": lens}
+        rev = new(B, T)
+        call("vtx_collate_tokens", flat, offs, cap.data_ptr(), rev.data_ptr(), lens.data_ptr(), B, T, max_len, pad, s)
+        if self.task == "captioning":
+            return {"caption_tokens": cap, "noitpac_tokens": rev, "caption_lengths": lens}
+        return {"labels": cap}

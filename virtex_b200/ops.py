@@ -62,6 +62,7 @@ _PROTOS = {
     "vtx_image_gray_sum": [P, P, P, P, I, I, P],
     "vtx_image_jitter_normalize": [P, P, P, P, P, P, I, I, P],
     "vtx_collate_tokens": [P, P, P, P, P, I, I, I, I64, P],
+    "vtx_collate_masked_lm": [P, P, P, P, P, I, I, I, I64, I64, I64, D, D, D, P, P],
     "vtx_jpeg_unstuff": [P, P, P, I, P, P, P, P, P, P, I, P],
     "vtx_jpeg_sync": [P, P, P, P, P, P, P, P, I, I, P, P, I, P, I, P],
     "vtx_jpeg_count_scan": [P, P, P, P, I, P],

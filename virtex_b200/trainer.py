@@ -24,6 +24,7 @@ import torch.distributed as dist
 from . import ops
 from .config import Config
 from .factories import param_group_hparams
+from .models import MaskedLMModel
 from .ops import _stream, call
 from .optim import lr_multiplier_fn
 
@@ -144,10 +145,17 @@ class Trainer:
         if self.model.engine is not eng:
             raise RuntimeError("the model rebuilt its engine (model.to() / .cuda() after Trainer construction): "
                                "create a new Trainer, this one would update a stale parameter arena")
-        eng.seed.add_(1)
         m = self.model
+        masked_lm = isinstance(m, MaskedLMModel)
+        if masked_lm and "masked_labels" not in batch:  # without them the loss would be next-token prediction
+            raise KeyError("a masked-LM batch carries 'masked_labels' (GpuInputPipeline with task='masked_lm')")
+        eng.seed.add_(1)
         if eng.classify:  # token / multilabel classification: loss slots [loss, 0]
             loss = eng.forward(batch["image"], None, None, None, training=True, with_grad=True, labels=batch["labels"])
+        elif masked_lm:  # one direction, cross entropy at the labelled positions: loss slots [loss, 0]
+            tokens = batch["caption_tokens"]
+            loss = eng.forward(batch["image"], tokens, tokens, batch["caption_lengths"], training=True, with_grad=True,
+                               labels=batch["masked_labels"])
         else:
             loss = eng.forward(batch["image"], batch["caption_tokens"],
                                batch["noitpac_tokens"] if m.caption_backward else batch["caption_tokens"],
