@@ -221,8 +221,15 @@ int vtx_add_ln_fwd(const float* res, const void* branch, const float* gamma, con
 int vtx_ln_bwd(const float* dy_a, const void* dy_b, const float* z, const float* stats, const float* gamma,
                const float* d_skip, float* d_res, void* d_branch, float* d_gamma, float* d_beta, int M, int H, float p,
                const uint64_t* seed, uint32_t site, int ln, void* stream);
-/* attention core, head_dim 64, Tq <= 32, Tk <= 64; causal = 1: key j visible to query i iff j <= i and j < lengths[b];
-   causal = 2: iff j < lengths[b] (key-padding mask only: masked language modelling); causal = 0: every key */
+/* Attention core, head_dim 64, 1 <= Tq, Tk <= VTX_ATTN_MAX_T (larger shapes: VTX_EINVAL); bf16 q / k / v / out with
+   leading dimensions that are multiples of 8.  causal = 1: key j visible to query i iff j <= i and j < lengths[b];
+   causal = 2: iff j < lengths[b] (key-padding mask only: masked language modelling); causal = 0: every key.
+   With Qs = Tq rounded up to a multiple of 32 and Ks = Tk rounded up to a multiple of 64, `lse` holds B * heads * Qs
+   fp32 rows (row (b * heads + h) * Qs + i; rows i >= Tq are not written) and the dropout mask of the probabilities is
+   the counter hash of element ((b * heads + h) * Qs + i) * Ks + j.  Tq <= 32 and Tk <= 64 run on one warp per
+   (b, h); longer shapes stream 64-row tiles (one CTA per (b, h, 64 queries) forward, per (b, h) backward).  Both are
+   deterministic and allocate nothing. */
+#define VTX_ATTN_MAX_T 1024
 int vtx_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out,
                  int64_t ldo, float* lse, int B, int heads, int Tq, int Tk, const int64_t* lengths, int causal,
                  float p, const uint64_t* seed, uint32_t site, void* stream);

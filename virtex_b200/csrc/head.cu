@@ -884,6 +884,409 @@ __global__ void __launch_bounds__(32 * kAttnBwdWarps) attn_bwd_kernel(const Attn
   }
 }
 
+// ------------------------------------------------------------------------------------------------ long attention
+// Shapes past the one-warp kernels (Tq > 32 or Tk > 64, each <= VTX_ATTN_MAX_T): larger crops give more visual keys,
+// longer captions more queries and keys.  A CTA of 4 warps streams 64-row tiles of K|V (or Q|dO) through a
+// double-buffered cp.async ring; each warp owns 16 rows of every tile, the products are the same mma.sync tiles.
+//   * forward, one CTA per (b, h, 64 queries): pass 1 over the key tiles finds each row's max and sum; pass 2
+//     recomputes S and accumulates P V with P = exp(S - max) rounded to bf16 after dropout, exactly as the one-warp
+//     kernel rounds it, and divides by the sum at the end;
+//   * backward, one CTA per (b, h), no scratch and no atomics: for every query tile, D_i = sum_j P_ij dP_ij over all
+//     key tiles (kept in shared memory, at most VTX_ATTN_MAX_T floats), then dQ = dS K over the key tiles again; then
+//     for every key tile, dV = Pd^T dO and dK = dS^T Q over the query tiles, Pd and dS staged as bf16 [query][key].
+// Key tiles no query of the tile can see (causal, key padding) are skipped; their dK, dV rows are written as zeros.
+// Dropout index ((b * heads + h) * Qs + i) * Ks + j and LSE row (b * heads + h) * Qs + i, Qs = Tq rounded up to 32,
+// Ks = Tk rounded up to 64: the one-warp kernels' layout (Qs = 32, Ks = 64) wherever they apply.
+constexpr int kLongWarps = 4;
+constexpr int kLongRows = 16 * kLongWarps;  // rows of one staged tile
+constexpr int kTile = kLongRows * kLd;      // bf16 elements of one staged tile
+constexpr int kAttnLongFwdSmem = 5 * kTile * 2;                              // Q + 2 stages of K, V
+constexpr int kAttnLongBwdSmem = 8 * kTile * 2 + VTX_ATTN_MAX_T * 4;          // 2 fixed + 2 x 2 streamed + Pd, dS; D
+
+__host__ __device__ __forceinline__ int attn_rows_q(int Tq) { return (Tq + 31) & ~31; }
+__host__ __device__ __forceinline__ int attn_rows_k(int Tk) { return (Tk + 63) & ~63; }
+
+// warp `warp` stages its 16 rows of a 64-row tile whose first `rows` rows exist (rows may be <= 0: all zero-filled)
+__device__ __forceinline__ void stage_tile_async(__nv_bfloat16* dst, const __nv_bfloat16* src, long long ld, int rows,
+                                                 int warp, int lane) {
+  const int r0 = warp * 16;
+  stage_rows_async(dst + r0 * kLd, src + (rows > r0 ? (long long)r0 * ld : 0), ld, rows - r0, 16, lane);
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ bool attn_allowed(const AttnArgs& a, int i, int j, int len) {
+  return i < a.Tq && j < a.Tk && (a.causal == 1 ? (j <= i && j < len) : a.causal == 2 ? (j < len) : true);
+}
+// keys [0, end) can be visible to the queries [q0, q1)
+__device__ __forceinline__ int attn_key_end(const AttnArgs& a, int len, int q1) {
+  const int e = a.causal ? min(len, a.Tk) : a.Tk;
+  return a.causal == 1 ? min(e, min(q1, a.Tq)) : e;
+}
+// s[nt] (16 rows x 64 keys of a warp) = A B^T over head_dim, A from 4 k-step fragments, B a [key][d] tile
+__device__ __forceinline__ void attn_scores(float (*s)[4], const uint32_t (*af)[4], const __nv_bfloat16* tB, int lane) {
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) s[nt][e] = 0.f;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      uint32_t bf[2];
+      frag_b(bf, tB, nt * 8, ks * 16, lane);
+      mma16816(s[nt], af[ks], bf);
+    }
+}
+// acc[nt] (16 rows x 64 columns) += X T, X the warp's 16 x 64 register tile (bf16-rounded), T a [64][d] smem tile
+__device__ __forceinline__ void attn_acc_xt(float (*acc)[4], const float (*x)[4], const __nv_bfloat16* t, int lane) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    uint32_t pf[4];
+    pf[0] = pack_bf2(x[2 * ks][0], x[2 * ks][1]);
+    pf[1] = pack_bf2(x[2 * ks][2], x[2 * ks][3]);
+    pf[2] = pack_bf2(x[2 * ks + 1][0], x[2 * ks + 1][1]);
+    pf[3] = pack_bf2(x[2 * ks + 1][2], x[2 * ks + 1][3]);
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      uint32_t bf[2];
+      frag_b_t(bf, t, ks * 16, nt * 8, lane);
+      mma16816(acc[nt], pf, bf);
+    }
+  }
+}
+__device__ __forceinline__ void load_frags_a(uint32_t (*af)[4], const __nv_bfloat16* t, int m0, int lane) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) frag_a(af[ks], t, m0, ks * 16, lane);
+}
+__device__ __forceinline__ void store_rows16(__nv_bfloat16* base, long long ld, int row0, int rows, const float (*acc)[4],
+                                             int lane) {
+  const int g = lane >> 2, tq = lane & 3;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int r = row0 + g + hh * 8;
+    if (r >= rows) continue;
+    __nv_bfloat16* op = base + (long long)r * ld + 2 * tq;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt)
+      *reinterpret_cast<uint32_t*>(op + nt * 8) = pack_bf2(acc[nt][hh * 2], acc[nt][hh * 2 + 1]);
+  }
+}
+
+__global__ void __launch_bounds__(32 * kLongWarps) attn_fwd_long_kernel(const AttnArgs a, __nv_bfloat16* __restrict__ out,
+                                                                          long long ldo, float* __restrict__ lse) {
+  VTX_PDL_TRIGGER();
+  const uint64_t seed = a.seed_ptr ? *a.seed_ptr : 0ull;
+  extern __shared__ __align__(16) uint8_t sm_raw[];
+  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(sm_raw);
+  __nv_bfloat16* sKV = sQ + kTile;  // stage s: K at sKV + 2 s kTile, V after it
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
+  const int unit = blockIdx.x, b = unit / a.heads, h = unit % a.heads;
+  const int q0 = blockIdx.y * kLongRows, r0 = q0 + 16 * warp;
+  const long long Qs = attn_rows_q(a.Tq), Ks = attn_rows_k(a.Tk);
+  const int len = a.causal ? (int)a.lengths[b] : a.Tk;
+  const int nkb = max(1, (attn_key_end(a, len, q0 + kLongRows) + kLongRows - 1) / kLongRows);
+  const __nv_bfloat16* kp = a.k + (long long)b * a.Tk * a.ldk + h * kD;
+  const __nv_bfloat16* vp = a.v + (long long)b * a.Tk * a.ldv + h * kD;
+  // steps 0 .. nkb-1: pass 1 (K tiles); nkb .. 2 nkb - 1: pass 2 (K and V tiles)
+  auto stage = [&](int step) {
+    const int kb = step < nkb ? step : step - nkb;
+    __nv_bfloat16* dst = sKV + (step & 1) * 2 * kTile;
+    stage_tile_async(dst, kp + (long long)kb * kLongRows * a.ldk, a.ldk, a.Tk - kb * kLongRows, warp, lane);
+    if (step >= nkb)
+      stage_tile_async(dst + kTile, vp + (long long)kb * kLongRows * a.ldv, a.ldv, a.Tk - kb * kLongRows, warp, lane);
+  };
+  stage_tile_async(sQ, a.q + ((long long)b * a.Tq + q0) * a.ldq + h * kD, a.ldq, a.Tq - q0, warp, lane);
+  stage(0);
+  cp_async_commit();
+  const float inv_keep = a.p > 0.f ? 1.f / (1.f - a.p) : 1.f;
+  const bool active = r0 < a.Tq;
+  uint32_t qf[4][4];
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[8][4];
+#pragma unroll
+  for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
+  for (int step = 0; step < 2 * nkb; ++step) {
+    if (step + 1 < 2 * nkb) {
+      stage(step + 1);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    if (step == 0) load_frags_a(qf, sQ, 16 * warp, lane);
+    if (active) {
+      const int kb = step < nkb ? step : step - nkb;
+      const __nv_bfloat16* sK = sKV + (step & 1) * 2 * kTile;
+      float s[8][4];
+      attn_scores(s, qf, sK, lane);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int i = r0 + g + hh * 8;
+        float mx = -INFINITY;
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = kb * kLongRows + nt * 8 + 2 * tq + e;
+            const float v = attn_allowed(a, i, j, len) ? s[nt][hh * 2 + e] * a.scale : -INFINITY;
+            s[nt][hh * 2 + e] = v;
+            mx = fmaxf(mx, v);
+          }
+        if (step < nkb) {  // pass 1: running max and sum (the scores are recomputed in pass 2)
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          const float mn = fmaxf(m[hh], mx);
+          const float mu = mn == -INFINITY ? 0.f : mn;  // no key yet (rows i >= Tq: never): l stays 0
+          float sum = 0.f;
+#pragma unroll
+          for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v = s[nt][hh * 2 + e];
+              sum += (v == -INFINITY) ? 0.f : __expf(v - mu);
+            }
+          // every lane of the warp shuffles: the rows of one warp differ in whether they have a visible key
+          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+          l[hh] = l[hh] * __expf(m[hh] - mu) + sum;
+          m[hh] = mn;
+        } else {  // pass 2: dropped, unnormalised probabilities against the row's final max
+#pragma unroll
+          for (int nt = 0; nt < 8; ++nt) {
+            const int j = kb * kLongRows + nt * 8 + 2 * tq;
+            const Drop4 dr = drop4(a.p, inv_keep, seed, a.site, (((uint64_t)unit * Qs + i) * Ks + j) >> 2);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v = s[nt][hh * 2 + e];
+              s[nt][hh * 2 + e] = ((v == -INFINITY) ? 0.f : __expf(v - m[hh])) * dr.scale(((2 * tq) & 3) + e);
+            }
+          }
+        }
+      }
+      if (step >= nkb) attn_acc_xt(o, s, sK + kTile, lane);
+    }
+    __syncthreads();
+  }
+  if (!active) return;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int i = r0 + g + hh * 8;
+    if (i >= a.Tq) continue;
+    if (tq == 0 && lse) lse[unit * Qs + i] = m[hh] + __logf(l[hh]);
+    const float inv = 1.f / l[hh];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      o[nt][hh * 2] *= inv;
+      o[nt][hh * 2 + 1] *= inv;
+    }
+  }
+  store_rows16(out + (long long)b * a.Tq * ldo + h * kD, ldo, r0, a.Tq, o, lane);
+}
+
+// P (dropout scale in pm) and dS of the warp's 16 x 64 tile at query row r0, key column k0, from S (in s, scaled
+// scores) and dPd (in dp); D of the rows in d[2] (ignored when !want_ds).  Returns the rows' sum of P dP in dsum.
+__device__ __forceinline__ void attn_bwd_probs(const AttnArgs& a, float (*s)[4], float (*dp)[4], const float* lse,
+                                               long long unit, long long Qs, long long Ks, int r0, int k0, int len,
+                                               uint64_t seed, float inv_keep, const float* d, float* dsum, int lane) {
+  const int g = lane >> 2, tq = lane & 3;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int i = r0 + g + hh * 8;
+    const float L = i < a.Tq ? lse[unit * Qs + i] : 0.f;
+    float Di = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const int j0 = k0 + nt * 8 + 2 * tq;
+      const Drop4 dr = drop4(a.p, inv_keep, seed, a.site, ((unit * Qs + i) * Ks + j0) >> 2);
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float pr = attn_allowed(a, i, j0 + e, len) ? __expf(s[nt][hh * 2 + e] * a.scale - L) : 0.f;
+        const float mk = dr.scale(((2 * tq) & 3) + e);
+        const float dpr = dp[nt][hh * 2 + e] * mk;
+        Di += pr * dpr;
+        s[nt][hh * 2 + e] = pr * mk;                               // Pd
+        dp[nt][hh * 2 + e] = pr * (dpr - d[hh]) * a.scale;         // dS
+      }
+    }
+    Di += __shfl_xor_sync(0xffffffffu, Di, 1);
+    Di += __shfl_xor_sync(0xffffffffu, Di, 2);
+    dsum[hh] = Di;
+  }
+}
+
+__global__ void __launch_bounds__(32 * kLongWarps) attn_bwd_long_kernel(const AttnArgs a, const __nv_bfloat16* __restrict__ dout,
+                                                                          long long ldo, const float* __restrict__ lse,
+                                                                          __nv_bfloat16* __restrict__ dq, long long lddq,
+                                                                          __nv_bfloat16* __restrict__ dk, long long lddk,
+                                                                          __nv_bfloat16* __restrict__ dv, long long lddv) {
+  VTX_PDL_TRIGGER();
+  const uint64_t seed = a.seed_ptr ? *a.seed_ptr : 0ull;
+  extern __shared__ __align__(16) uint8_t sm_raw[];
+  __nv_bfloat16* sF = reinterpret_cast<__nv_bfloat16*>(sm_raw);  // fixed pair: Q, dO (phase 1) or K, V (phase 2)
+  __nv_bfloat16* sS = sF + 2 * kTile;                              // streamed pairs, 2 stages
+  __nv_bfloat16* sP = sS + 4 * kTile;                              // Pd [query][key] (phase 2)
+  __nv_bfloat16* sdS = sP + kTile;                                 // dS [query][key] (phase 2)
+  float* sD = reinterpret_cast<float*>(sdS + kTile);               // D of every query row
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
+  const long long unit = blockIdx.x;
+  const int b = (int)(unit / a.heads), h = (int)(unit % a.heads);
+  const long long Qs = attn_rows_q(a.Tq), Ks = attn_rows_k(a.Tk);
+  const int len = a.causal ? (int)a.lengths[b] : a.Tk;
+  const float inv_keep = a.p > 0.f ? 1.f / (1.f - a.p) : 1.f;
+  const __nv_bfloat16* qp = a.q + (long long)b * a.Tq * a.ldq + h * kD;
+  const __nv_bfloat16* op = dout + (long long)b * a.Tq * ldo + h * kD;
+  const __nv_bfloat16* kp = a.k + (long long)b * a.Tk * a.ldk + h * kD;
+  const __nv_bfloat16* vp = a.v + (long long)b * a.Tk * a.ldv + h * kD;
+  const int nqb = (a.Tq + kLongRows - 1) / kLongRows;
+  const int kend_all = attn_key_end(a, len, a.Tq);
+  const int nkb_all = (a.Tk + kLongRows - 1) / kLongRows;
+  // ---- phase 1, per query tile: D over the key tiles (pass 1), then dQ = dS K over them again (pass 2)
+  for (int qb = 0; qb < nqb; ++qb) {
+    const int q0 = qb * kLongRows, r0 = q0 + 16 * warp;
+    const int nkb = max(1, (attn_key_end(a, len, q0 + kLongRows) + kLongRows - 1) / kLongRows);
+    auto stage = [&](int step) {
+      const int kb = step < nkb ? step : step - nkb;
+      __nv_bfloat16* dst = sS + (step & 1) * 2 * kTile;
+      stage_tile_async(dst, kp + (long long)kb * kLongRows * a.ldk, a.ldk, a.Tk - kb * kLongRows, warp, lane);
+      stage_tile_async(dst + kTile, vp + (long long)kb * kLongRows * a.ldv, a.ldv, a.Tk - kb * kLongRows, warp, lane);
+    };
+    stage_tile_async(sF, qp + (long long)q0 * a.ldq, a.ldq, a.Tq - q0, warp, lane);
+    stage_tile_async(sF + kTile, op + (long long)q0 * ldo, ldo, a.Tq - q0, warp, lane);
+    stage(0);
+    cp_async_commit();
+    const bool active = r0 < a.Tq;
+    uint32_t qf[4][4], of[4][4];
+    float D[2] = {0.f, 0.f};
+    float acc[8][4];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
+    for (int step = 0; step < 2 * nkb; ++step) {
+      if (step + 1 < 2 * nkb) {
+        stage(step + 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+      } else {
+        cp_async_wait<0>();
+      }
+      __syncthreads();
+      if (step == 0) {
+        load_frags_a(qf, sF, 16 * warp, lane);
+        load_frags_a(of, sF + kTile, 16 * warp, lane);
+      }
+      if (active) {
+        const int kb = step < nkb ? step : step - nkb;
+        const __nv_bfloat16* sK = sS + (step & 1) * 2 * kTile;
+        float s[8][4], dp[8][4], dsum[2];
+        attn_scores(s, qf, sK, lane);
+        attn_scores(dp, of, sK + kTile, lane);
+        attn_bwd_probs(a, s, dp, lse, unit, Qs, Ks, r0, kb * kLongRows, len, seed, inv_keep, D, dsum, lane);
+        if (step < nkb) {
+          D[0] += dsum[0];
+          D[1] += dsum[1];
+        } else {
+          attn_acc_xt(acc, dp, sK, lane);
+        }
+      }
+      __syncthreads();
+    }
+    if (active) {
+      store_rows16(dq + (long long)b * a.Tq * lddq + h * kD, lddq, r0, a.Tq, acc, lane);
+      if (tq == 0) {
+        sD[r0 + g] = D[0];
+        sD[r0 + g + 8] = D[1];
+      }
+    }
+  }
+  __syncthreads();
+  // ---- phase 2, per key tile: dV = Pd^T dO and dK = dS^T Q over the query tiles that can see it
+  for (int kb = 0; kb < nkb_all; ++kb) {
+    const int k0 = kb * kLongRows;
+    const int qb0 = a.causal == 1 ? k0 / kLongRows : 0;  // causal: query i sees key j only if i >= j
+    const int nsteps = k0 < kend_all ? nqb - qb0 : 0;
+    auto stage = [&](int step) {
+      const int q0 = (qb0 + step) * kLongRows;
+      __nv_bfloat16* dst = sS + (step & 1) * 2 * kTile;
+      stage_tile_async(dst, qp + (long long)q0 * a.ldq, a.ldq, a.Tq - q0, warp, lane);
+      stage_tile_async(dst + kTile, op + (long long)q0 * ldo, ldo, a.Tq - q0, warp, lane);
+    };
+    if (nsteps > 0) {
+      stage_tile_async(sF, kp + (long long)k0 * a.ldk, a.ldk, a.Tk - k0, warp, lane);
+      stage_tile_async(sF + kTile, vp + (long long)k0 * a.ldv, a.ldv, a.Tk - k0, warp, lane);
+      stage(0);
+      cp_async_commit();
+    }
+    float ak[8][4], av[8][4];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) ak[nt][e] = av[nt][e] = 0.f;
+    for (int step = 0; step < nsteps; ++step) {
+      if (step + 1 < nsteps) {
+        stage(step + 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+      } else {
+        cp_async_wait<0>();
+      }
+      __syncthreads();
+      const int q0 = (qb0 + step) * kLongRows, r0 = q0 + 16 * warp;
+      const __nv_bfloat16* tQ = sS + (step & 1) * 2 * kTile;
+      const __nv_bfloat16* tO = tQ + kTile;
+      {
+        uint32_t af[4][4];
+        float s[8][4], dp[8][4], dsum[2];
+        load_frags_a(af, tQ, 16 * warp, lane);
+        attn_scores(s, af, sF, lane);
+        load_frags_a(af, tO, 16 * warp, lane);
+        attn_scores(dp, af, sF + kTile, lane);
+        float d[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int i = r0 + g + hh * 8;
+          d[hh] = i < a.Tq ? sD[i] : 0.f;
+        }
+        attn_bwd_probs(a, s, dp, lse, unit, Qs, Ks, r0, k0, len, seed, inv_keep, d, dsum, lane);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int il = 16 * warp + g + hh * 8;
+#pragma unroll
+          for (int nt = 0; nt < 8; ++nt) {
+            *reinterpret_cast<uint32_t*>(sP + il * kLd + nt * 8 + 2 * tq) = pack_bf2(s[nt][hh * 2], s[nt][hh * 2 + 1]);
+            *reinterpret_cast<uint32_t*>(sdS + il * kLd + nt * 8 + 2 * tq) =
+                pack_bf2(dp[nt][hh * 2], dp[nt][hh * 2 + 1]);
+          }
+        }
+      }
+      __syncthreads();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        uint32_t ap[4], as_[4];
+        frag_a_t(ap, sP, 16 * warp, ks * 16, lane);
+        frag_a_t(as_, sdS, 16 * warp, ks * 16, lane);
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          uint32_t bo[2], bq[2];
+          frag_b_t(bo, tO, ks * 16, nt * 8, lane);
+          frag_b_t(bq, tQ, ks * 16, nt * 8, lane);
+          mma16816(av[nt], ap, bo);
+          mma16816(ak[nt], as_, bq);
+        }
+      }
+      __syncthreads();
+    }
+    store_rows16(dk + (long long)b * a.Tk * lddk + h * kD, lddk, k0 + 16 * warp, a.Tk, ak, lane);
+    store_rows16(dv + (long long)b * a.Tk * lddv + h * kD, lddv, k0 + 16 * warp, a.Tk, av, lane);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ GELU + dropout
 __global__ void gelu_dropout_fwd_kernel(const __nv_bfloat16* __restrict__ u, __nv_bfloat16* __restrict__ h,
                                         long long n8, float p, const uint64_t* seed_ptr, uint32_t site) {
@@ -1309,11 +1712,15 @@ extern "C" int vtx_ln_bwd(const float* dy_a, const void* dy_b, const float* z, c
   return check_launch("ln_bwd");
 }
 
+// the one-warp kernels keep every shape they take; the long kernels take the rest
+static bool attn_long(int Tq, int Tk) { return Tq > 32 || Tk > 64; }
+
 static int fill_attn(AttnArgs* a, const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                      int B, int heads, int Tq, int Tk, const int64_t* lengths, int causal, float p, const uint64_t* seed_ptr,
                      uint32_t site) {
-  if (!q || !k || !v || Tq < 1 || Tq > 32 || Tk < 1 || Tk > 64 || causal < 0 || causal > 2 || (causal && !lengths))
-    return set_error(VTX_EINVAL, "attention: unsupported shape (Tq<=32, Tk<=64, head_dim 64)");
+  if (!q || !k || !v || Tq < 1 || Tq > VTX_ATTN_MAX_T || Tk < 1 || Tk > VTX_ATTN_MAX_T || causal < 0 || causal > 2 ||
+      (causal && !lengths))
+    return set_error(VTX_EINVAL, "attention: unsupported shape (1 <= Tq, Tk <= VTX_ATTN_MAX_T, head_dim 64)");
   if (ldq % 8 || ldk % 8 || ldv % 8) return set_error(VTX_EINVAL, "attention: leading dims must be multiples of 8");
   a->q = (const __nv_bfloat16*)q; a->k = (const __nv_bfloat16*)k; a->v = (const __nv_bfloat16*)v;
   a->ldq = ldq; a->ldk = ldk; a->ldv = ldv;
@@ -1331,11 +1738,17 @@ extern "C" int vtx_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t l
   int rc = fill_attn(&a, q, ldq, k, ldk, v, ldv, B, heads, Tq, Tk, lengths, causal, p, seed_ptr, site);
   if (rc) return rc;
   REQ(out && ldo % 8 == 0, "bad output");
+  const int units = B * heads;
+  if (attn_long(Tq, Tk)) {
+    cudaFuncSetAttribute(attn_fwd_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongFwdSmem);
+    attn_fwd_long_kernel<<<dim3(units, (Tq + kLongRows - 1) / kLongRows), 32 * kLongWarps, kAttnLongFwdSmem, STREAM>>>(
+        a, (__nv_bfloat16*)out, ldo, lse);
+    return check_launch("attn_fwd_long");
+  }
   const size_t smem = (size_t)kAttnFwdWarps * attn_fwd_smem_per_warp((Tk + 15) & ~15);
   // per device and cheap: set unconditionally (a process may drive several devices through the module-level API)
   cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                        kAttnFwdWarps * attn_fwd_smem_per_warp(64));
-  const int units = B * heads;
   attn_fwd_kernel<<<(units + kAttnFwdWarps - 1) / kAttnFwdWarps, 32 * kAttnFwdWarps, smem, STREAM>>>(
       a, (__nv_bfloat16*)out, ldo, lse);
   return check_launch("attn_fwd");
@@ -1348,10 +1761,17 @@ extern "C" int vtx_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t l
   int rc = fill_attn(&a, q, ldq, k, ldk, v, ldv, B, heads, Tq, Tk, lengths, causal, p, seed_ptr, site);
   if (rc) return rc;
   REQ(dout && lse && dq && dk && dv && ldo % 8 == 0 && lddq % 8 == 0 && lddk % 8 == 0 && lddv % 8 == 0, "bad arguments");
+  const int units = B * heads;
+  if (attn_long(Tq, Tk)) {
+    cudaFuncSetAttribute(attn_bwd_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongBwdSmem);
+    attn_bwd_long_kernel<<<units, 32 * kLongWarps, kAttnLongBwdSmem, STREAM>>>(
+        a, (const __nv_bfloat16*)dout, ldo, lse, (__nv_bfloat16*)dq, lddq, (__nv_bfloat16*)dk, lddk, (__nv_bfloat16*)dv,
+        lddv);
+    return check_launch("attn_bwd_long");
+  }
   const size_t smem = (size_t)kAttnBwdWarps * attn_bwd_smem_per_warp((Tk + 15) & ~15);
   cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                        kAttnBwdWarps * attn_bwd_smem_per_warp(64));
-  const int units = B * heads;
   attn_bwd_kernel<<<(units + kAttnBwdWarps - 1) / kAttnBwdWarps, 32 * kAttnBwdWarps, smem, STREAM>>>(
       a, (const __nv_bfloat16*)dout, ldo, lse, (__nv_bfloat16*)dq, lddq, (__nv_bfloat16*)dk, lddk, (__nv_bfloat16*)dv,
       lddv);

@@ -30,6 +30,28 @@ from .ops import call, gemm, _p, _stream
 BF16, F32 = torch.bfloat16, torch.float32
 _ALIGN = 64  # arena alignment in elements (256 B for fp32, 128 B for bf16: TMA base pointers need 16 B)
 DECODE_MAX_KEYS = 64  # VTX_DECODE_MAX_KEYS of include/virtex_b200.h
+ATTN_MAX_T = 1024  # VTX_ATTN_MAX_T: queries and keys per (image, head) of vtx_attn_fwd / _bwd
+
+
+def _feature_grid(h, w):
+    """(h, w) of the backbone's output for an h x w image: the stem conv, max-pool and layer2..4 each map x to
+    (x - 1) // 2 + 1 (8 x 8 for 256 x 256, 10 x 10 for 320 x 320)."""
+    for _ in range(5):
+        h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    return h, w
+
+
+def _check_attention(T, hw):
+    """Raises before any launch when a caption of T tokens or h * w = hw feature positions exceed the attention
+    kernels (self-attention: T queries and keys; cross-attention: T queries, hw keys)."""
+    if T > ATTN_MAX_T or hw > ATTN_MAX_T:
+        raise ValueError(f"attention takes at most {ATTN_MAX_T} queries and keys per image and head: got captions of "
+                         f"{T} tokens and {hw} feature positions")
+
+
+def _lse_rows(B, A, T):
+    """fp32 log-sum-exp rows vtx_attn_fwd writes for T queries: B * A * (T rounded up to 32)."""
+    return B * A * _round_up(T, 32)
 
 
 def _round_up(x, m):
@@ -818,7 +840,7 @@ class Engine:
         qkv = self.ws.get(k + "qkv", (M, 3 * H), BF16)
         gemm(x, self.W(q + "in_proj_weight"), qkv, M, 3 * H, H, bias=self.P(q + "in_proj_bias"))
         o = self.ws.get(k + "o_s", (M, H), BF16)
-        lse = self.ws.get(k + "lse_s", (rec["B"] * rec["A"] * 32,), F32)
+        lse = self.ws.get(k + "lse_s", (_lse_rows(rec["B"], rec["A"], rec["T"]),), F32)
         self._attn_fwd(rec, *qkv.split(H, 1), o, lse, rec["T"], rec["lengths"], rec["mask_mode"], lr["sb"])
         gemm(o, self.W(q + "out_proj.weight"), out, M, H, H, bias=self.P(q + "out_proj.bias"))
         lr.update(x_s=x, qkv=qkv, o_s=o, lse_s=lse)
@@ -840,7 +862,7 @@ class Engine:
         kv = self.ws.get(k + "kv", (S, 2 * H), BF16)
         gemm(rec["mem"], w[H:], kv, S, 2 * H, H, bias=b[H:])
         o = self.ws.get(k + "o_c", (M, H), BF16)
-        lse = self.ws.get(k + "lse_c", (rec["B"] * rec["A"] * 32,), F32)
+        lse = self.ws.get(k + "lse_c", (_lse_rows(rec["B"], rec["A"], rec["T"]),), F32)
         self._attn_fwd(rec, qc, *kv.split(H, 1), o, lse, rec["Sk"], None, 0, lr["sb"] + 2)
         gemm(o, self.W(q + "out_proj.weight"), out, M, H, H, bias=self.P(q + "out_proj.bias"))
         lr.update(x_c=x, qc=qc, kv=kv, o_c=o, lse_c=lse)
@@ -1033,6 +1055,8 @@ class Engine:
         self.generation += 1
         self.loss.zero_()
         self.count.zero_()
+        if not self.classify:  # an NCHW image fixes the backbone's h x w grid: check the attention shapes up front
+            _check_attention(tokens.shape[1], math.prod(_feature_grid(*image.shape[2:])) if image.dim() == 4 else 0)
         # BatchNorm follows the backbone's OWN mode flag, like the reference's nn.BatchNorm2d: `model.train()` puts a
         # frozen backbone's BN back into batch-statistics mode (visual_backbones.py:48-52 only calls .eval() once)
         bn_training = bool(self.visual.cnn.training) if self.visual is not None else training
@@ -1143,9 +1167,7 @@ class Engine:
             raise ValueError(f"{what} needs {positions} positions; the head has {mod.max_caption_length}")
         # vtx_attn_decode attends over at most DECODE_MAX_KEYS keys: the self-attention cache slots and the h * w
         # feature positions of cross-attention (h = w = 8 for a 256 x 256 image)
-        h, w = image.shape[2], image.shape[3]
-        for _ in range(5):  # stem conv, max-pool, layer2..4: each (x - 1) // 2 + 1
-            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        h, w = _feature_grid(image.shape[2], image.shape[3])
         if positions > DECODE_MAX_KEYS or h * w > DECODE_MAX_KEYS:
             raise ValueError(f"{what} attends over at most {DECODE_MAX_KEYS} keys: it needs {positions} positions, a "
                              f"{image.shape[2]} x {image.shape[3]} image {h * w} feature positions")
@@ -1488,10 +1510,11 @@ def resnet_forward(cnn, image: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def head_logits(head, visual_features, caption_tokens, caption_lengths) -> torch.Tensor:
     """`TransformerDecoderTextualHead.forward`: (B,C,h,w), (B,T), (B,) -> fp32 logits (B,T,V)."""
+    B, C, h, w = visual_features.shape
+    _check_attention(caption_tokens.shape[1], h * w)
     eng = _module_engine(head, textual=head)
     eng.mark_weights_dirty()
     eng.prepare_weights()
-    B, C, h, w = visual_features.shape
     feat = visual_features.permute(0, 2, 3, 1).reshape(B * h * w, C).to(BF16).contiguous()
     mem = eng.visual_projection_forward(feat, B * h * w)
     rec = eng.head_forward("textual", mem, caption_tokens.contiguous(), caption_lengths.contiguous(),
