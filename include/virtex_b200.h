@@ -67,8 +67,8 @@ typedef struct VtxGemm {
      A is the activation [conv_n, conv_h, conv_w, conv_c]; M = n*h*w, K = 9*conv_c, B = weights [N, (kh,kw,c)].
      conv_wgrad = 1 swaps roles for the weight gradient (see gemm_tc.cu). */
   int32_t conv_n, conv_h, conv_w, conv_c;
-  int32_t conv_mode; /* 0 = plain GEMM, 1 = implicit fprop/dgrad gather on A (64->64 channel problems run the halo-reuse
-                        variant automatically), 2 = wgrad gather on B,
+  int32_t conv_mode; /* 0 = plain GEMM, 1 = implicit fprop/dgrad gather on A (any conv_c -> N, 3x3 / stride 1 or 2),
+                        2 = wgrad gather on B,
                         4 = wgrad for C = Cout = 64 in the transposed layout: A = dy, B = x, D[9*C, Cout] fp32 +=
                             (atomic), i.e. the TRANSPOSE of mode 2's [Cout, 9*C] output,
                         5 = 7x7/2 stem fprop over the space-to-depth view S written by vtx_stem_s2d: A = S
@@ -88,15 +88,18 @@ typedef struct VtxGemm {
      tile grid that fall outside the view are clipped. */
   int32_t conv_out_h, conv_out_w;
   int64_t ldd_w, ldd_h, ldd_n;
-  const uint8_t* residual_mask; /* optional (plain bf16 GEMMs, N % 32 == 0): bit (m, n) of a [M, N/8] bit mask in the layout
-                                   vtx_bn_act writes; residual[m, n] is added only where the bit is set.  This is the
-                                   shortcut gradient dz = dOut * [block output > 0] of a bottleneck without dz ever being
-                                   written to memory (torchvision resnet.py:160-161 backward). */
+  const uint8_t* residual_mask; /* optional (bf16 output, N % 32 == 0; a plain GEMM, or conv_mode 1 without an output
+                                   view, whose row m is the NHWC output pixel): bit (m, n) of a [M, N/8] bit mask in the
+                                   layout vtx_bn_act writes; residual[m, n] is added only where the bit is set.  This is
+                                   the shortcut gradient dz = dOut * [block output > 0] of a residual block without dz
+                                   ever being written to memory (torchvision resnet.py:100-103, 160-161 backward): the
+                                   1x1 conv1 dgrad of a bottleneck, the 3x3 conv1 dgrad of a basic block. */
   /* BatchNorm-backward reduction fused into the epilogue (bnr_y != NULL; bf16 output, N % 8 == 0, no bias / activation /
      stats): D is the gradient w.r.t. the output of a train-mode BN (+ReLU) whose pre-BN input is bnr_y (same geometry as
      D: leading dimension bnr_ldy, or D's view strides for conv_mode 1 output views) and whose forward parameters are
      bnr_bnp [4, N] = mean, invstd, scale, shift (vtx_bn_finalize).  With dz = D * mask, mask = bit (m, n) of bnr_mask
-     (layout of vtx_bn_act's mask, plain GEMMs only) or, when bnr_mask is NULL, [bnr_y * scale + shift > 0],
+     (layout of vtx_bn_act's mask; plain GEMMs, or conv_mode 1 without an output view, rows as for residual_mask) or,
+     when bnr_mask is NULL, [bnr_y * scale + shift > 0],
          bnr_sums[0, n] += sum_m dz[m, n],    bnr_sums[1, n] += sum_m dz[m, n] * (bnr_y[m, n] - mean[n]) * invstd[n]
      -- exactly what vtx_bn_bwd_reduce computes in a separate pass over D and y (torch batch_norm backward, first half);
      D itself is stored unmasked, vtx_bn_bwd_finalize_apply consumes the sums. */

@@ -2,9 +2,9 @@
 
     python scripts/bench_downstream.py [--arch resnet50] [--batch 256] [--iters 20] [--warmup 5] [--rounds 3]
 
-Eval-mode forward of a torchvision ResNet (`--arch`: resnet50, resnet101, resnet152, wide_resnet50_2 or
-wide_resnet101_2) at 224 x 224, three ways, alternated within one process so that clock and power drift hit
-all three alike:
+Eval-mode forward of a torchvision ResNet (`--arch`: resnet18, resnet34, resnet50, resnet101, resnet152,
+wide_resnet50_2 or wide_resnet101_2) at 224 x 224, three ways, alternated within one process so that clock and power
+drift hit all three alike:
   * infer     -- Engine.backbone_infer (eval BN folded into the GEMM epilogues);
   * forward   -- Engine.backbone_forward(training=False) (raw conv outputs, then a BN + ReLU (+ residual) pass each);
   * eager     -- the same torchvision model, channels_last, bf16 autocast, cuDNN.
@@ -47,11 +47,19 @@ def activation_bytes(cnn, B, H=224):
     for li in range(1, 5):
         for blk in getattr(cnn, f"layer{li}"):
             stride = blk.stride
-            width, C4 = blk.conv1.weight.shape[0], blk.conv3.weight.shape[0]
             Hn = (Hc - 1) // stride + 1
+            ds = blk.downsample is not None
+            if not hasattr(blk, "conv3"):  # basic block: conv1 (stride) x -> a1, conv2 a1 (+ shortcut) -> out
+                C = blk.conv1.weight.shape[0]
+                x, a1, out = B * Hc * Hc * Cin * e, B * Hn * Hn * C * e, B * Hn * Hn * C * e
+                infer += (x + a1) + (x + out if ds else 0) + (a1 + out + out)
+                fwd += (x + a1) + 2 * a1 + (a1 + out) + (x + out if ds else 0)
+                fwd += out + (out if ds else x) + out  # bn2 (+ downsample BN) + residual + ReLU pass
+                Hc, Cin = Hn, C
+                continue
+            width, C4 = blk.conv1.weight.shape[0], blk.conv3.weight.shape[0]
             x, a1, a2, out = B * Hc * Hc * Cin * e, B * Hc * Hc * width * e, B * Hn * Hn * width * e, \
                 B * Hn * Hn * C4 * e
-            ds = blk.downsample is not None
             # folded: conv1 x -> a1, conv2 a1 -> a2, [downsample x -> shortcut], conv3 a2 + shortcut -> out
             infer += (x + a1) + (a1 + a2) + (x + out if ds else 0) + (a2 + out + out)
             # unfused: every conv writes y and a BN pass reads it back and writes the activation (+ reads the shortcut)
@@ -84,22 +92,27 @@ def main():
         raise SystemExit("bench_downstream.py measures the GPU path: no CUDA device")
     import torchvision
     from virtex_b200.modules import ResNetParams
-    from tests import downstream_oracle as DO, wide_oracle as WO
+    from tests import basic_oracle as BO, downstream_oracle as DO, wide_oracle as WO
 
     print(f"card: {card()}", flush=True)
     torch.manual_seed(0)
     dev = torch.device("cuda")
+    width = ResNetParams(a.arch).out_channels
     if a.arch == "resnet50":
         state = DO.synth_state(0, a.classes)
     else:  # the same recipe on the other architecture's parameter tree
-        spec = WO.spec(a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
-        state = {k[len(DO.PREFIX):]: v for k, v in WO.synth_state(spec, 0, bn3_gain=0.25).items()
-                 if k.startswith(DO.PREFIX)}
+        if a.arch in BO.BLOCKS:
+            spec = BO.spec(a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
+            full = BO.synth_state(spec, 0, residual_gain=0.25)
+        else:
+            spec = WO.spec(a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
+            full = WO.synth_state(spec, 0, bn3_gain=0.25)
+        state = {k[len(DO.PREFIX):]: v for k, v in full.items() if k.startswith(DO.PREFIX)}
         g = torch.Generator().manual_seed(7000)
-        state["fc.weight"] = torch.randn(a.classes, 2048, generator=g) * 0.01
+        state["fc.weight"] = torch.randn(a.classes, width, generator=g) * 0.01
         state["fc.bias"] = torch.randn(a.classes, generator=g) * 0.1
     cnn = ResNetParams(a.arch)
-    cnn.fc = nn.Linear(2048, a.classes)
+    cnn.fc = nn.Linear(width, a.classes)
     cnn.load_state_dict(state, strict=True)
     cnn = cnn.to(dev).eval()
     image = torch.randn(a.batch, 3, 224, 224, device=dev)
@@ -128,8 +141,8 @@ def main():
         for k, fn in ways.items():
             times[k].append(timed(fn, a.iters))
     # same outputs: pooled features of the folded and the unfused engine forward
-    f1 = eng.backbone_infer(image)[0].float().view(a.batch, -1, 2048).mean(1)
-    f2 = eng.backbone_forward(image, training=False)[0].float().view(a.batch, -1, 2048).mean(1)
+    f1 = eng.backbone_infer(image)[0].float().view(a.batch, -1, width).mean(1)
+    f2 = eng.backbone_forward(image, training=False)[0].float().view(a.batch, -1, width).mean(1)
     pooled_rel = ((f1 - f2).norm() / f2.norm()).item()
 
     # linear probe: frozen eval-mode backbone, only fc trains
@@ -144,7 +157,7 @@ def main():
 
     # fine-tuning: train mode, every parameter
     ft = ResNetParams(a.arch)
-    ft.fc = nn.Linear(2048, a.classes)
+    ft.fc = nn.Linear(width, a.classes)
     ft.load_state_dict(state, strict=True)
     ft = ft.to(dev).train()
     opt_ft = torch.optim.SGD(ft.parameters(), lr=0.025, momentum=0.9, weight_decay=1e-4)

@@ -79,8 +79,9 @@ class Bicaptioning(nn.Module):
     def __init__(self, arch="resnet50", vocab=10000, hidden=1024, layers=1, heads=16, ffn=4096, dropout=0.1):
         super().__init__()
         self.cnn = getattr(torchvision.models, arch)(weights=None, zero_init_residual=True)
+        width = self.cnn.fc.in_features  # layer4's channels: 512 for resnet18/34, 2048 for the bottleneck ResNets
         self.cnn.fc = nn.Identity()
-        self.textual = Head(2048, vocab, hidden, layers, heads, ffn, dropout)
+        self.textual = Head(width, vocab, hidden, layers, heads, ffn, dropout)
         self.backward_textual = copy.deepcopy(self.textual)
         self.backward_textual.visual_projection = self.textual.visual_projection
         self.backward_textual.embedding = self.textual.embedding

@@ -817,6 +817,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int w = (tw << p.lbw) + dw, h = (th << p.lbh) + dh, n = (tn << p.lbn) + dn;
           ok = (w < p.vW) && (h < p.vH) && (n < p.cN);
           off = (uint32_t)n * (uint32_t)p.bnr_sn + (uint32_t)h * (uint32_t)p.bnr_sh + (uint32_t)w * (uint32_t)p.bnr_sw;
+          // the bit mask's row: the NHWC output pixel (the host allows the mask only without an output view)
+          lin = ((uint32_t)n * (uint32_t)p.cH + (uint32_t)h) * (uint32_t)p.cW + (uint32_t)w;
         } else {
           lin = (uint32_t)(mt * kBM + r);
           ok = lin < (uint32_t)p.M;
@@ -1147,19 +1149,22 @@ extern "C" int vtx_gemm(const VtxGemm* g, void* stream_) {
   p.bias_pairs = (g->bias != nullptr && g->N % 2 == 0 && (reinterpret_cast<uintptr_t>(g->bias) & 7) == 0) ? 1 : 0;
   p.residual = reinterpret_cast<const __nv_bfloat16*>(g->residual);
   p.ldr = g->ldr;
+  // the bit masks (residual_mask, bnr_mask) address row m of D: a plain GEMM's row, or a conv_mode 1 output's NHWC pixel
+  const bool mask_rows = g->conv_mode == 0 || (g->conv_mode == 1 && g->conv_out_w <= 0);
   p.res_mask = reinterpret_cast<const uint8_t*>(g->residual_mask);
-  if (p.res_mask != nullptr && (g->residual == nullptr || g->N % 32 != 0 || g->conv_mode != 0 || g->out_f32 ||
+  if (p.res_mask != nullptr && (g->residual == nullptr || g->N % 32 != 0 || !mask_rows || g->out_f32 ||
                                 (reinterpret_cast<uintptr_t>(g->residual_mask) & 3) != 0))
-    return set_error(VTX_EINVAL, "vtx_gemm: residual_mask needs a residual, a plain bf16 GEMM and N %% 32 == 0");
+    return set_error(VTX_EINVAL, "vtx_gemm: residual_mask needs a residual, a bf16 output of a plain GEMM or of conv_mode "
+                                 "1 without an output view, and N %% 32 == 0");
   p.stats = g->stats;
   const bool bnr = g->bnr_y != nullptr;
   if (bnr) {
     if (!g->bnr_bnp || !g->bnr_sums || g->stats || g->out_f32 || g->bias || g->act || (g->alpha != 0.f && g->alpha != 1.f) ||
         g->N % 8 != 0 || g->bnr_ldy % 8 != 0 || (reinterpret_cast<uintptr_t>(g->bnr_y) & 15) != 0 ||
-        (reinterpret_cast<uintptr_t>(g->bnr_bnp) & 15) != 0 || (g->bnr_mask != nullptr && g->conv_mode != 0) ||
+        (reinterpret_cast<uintptr_t>(g->bnr_bnp) & 15) != 0 || (g->bnr_mask != nullptr && !mask_rows) ||
         g->conv_mode == 2 || g->conv_mode >= 4 || split_k > 1)
       return set_error(VTX_EINVAL, "vtx_gemm: bnr needs a plain bf16 output (no stats/bias/activation/alpha/split-K), "
-                                   "N %% 8 == 0, 16-byte aligned y / bnp; the bit-mask form needs conv_mode 0");
+                                   "N %% 8 == 0, 16-byte aligned y / bnp; the bit-mask form needs conv_mode 0, or 1 without an output view");
     if ((long long)g->M * (g->bnr_ldy > g->N ? g->bnr_ldy : g->N) >= (1ll << 31))
       return set_error(VTX_EUNSUPPORTED, "vtx_gemm: bnr needs M * ld(y) < 2^31");
     p.stats = g->bnr_sums;

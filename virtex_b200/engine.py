@@ -24,7 +24,7 @@ import torch
 from torch import nn
 
 from . import ops
-from .modules import LinearTextualHead
+from .modules import BasicBlock, LinearTextualHead
 from .ops import call, gemm, _p, _stream
 
 BF16, F32 = torch.bfloat16, torch.float32
@@ -146,8 +146,24 @@ def _require_cuda(dev):
 
 def _block_widths(blk):
     """(inner width of conv1 / conv2, output width of conv3) of a bottleneck, read from its weights: 4x apart for
-    ResNet-50/101/152, 2x for the wide models."""
+    ResNet-50/101/152, 2x for the wide models.  A basic block's two 3x3 convs and its output share one width."""
+    if isinstance(blk, BasicBlock):
+        return blk.conv1.weight.shape[0], blk.conv2.weight.shape[0]
     return blk.conv1.weight.shape[0], blk.conv3.weight.shape[0]
+
+
+def _convs3x3(name, blk):
+    """(weight prefix, stride) of every 3x3 conv of block `name`: conv2 of a bottleneck; conv1 (strided) and conv2 of a
+    basic block."""
+    if isinstance(blk, BasicBlock):
+        return [(name + ".conv1", blk.stride), (name + ".conv2", 1)]
+    return [(name + ".conv2", blk.stride)]
+
+
+def _transposed_wgrad(Cin, C, stride):
+    """True when a 3x3 conv's weight gradient runs as conv_mode 4 (64 -> 64, stride 1), whose [(tap, cin), cout]
+    layout the unpack job of kind 3 reads; every other 3x3 wgrad is the split-K conv_mode 2 into [C, 9 * Cin]."""
+    return Cin == 64 and C == 64 and stride == 1
 
 
 class Engine:
@@ -225,7 +241,10 @@ class Engine:
         # fp32 weight-gradient scratch of every k > 1 convolution (GEMM output layout), one flat buffer zeroed once per
         # backward; the batched unpack jobs fold it into the OIHW gradient arena per all-reduce bucket
         sizes = [("visual.cnn.conv1", 64 * 256)]
-        sizes += [(name + ".conv2", 9 * blk.conv2.weight.shape[0] ** 2) for name, blk in self.blocks]
+        for name, blk in self.blocks:  # [C, 9 * Cin] per 3x3 conv: conv2, and a basic block's conv1
+            if isinstance(blk, BasicBlock):
+                sizes.append((name + ".conv1", blk.conv1.weight.numel()))
+            sizes.append((name + ".conv2", blk.conv2.weight.numel()))
         total = sum(_round_up(n, _ALIGN) for _, n in sizes)
         self._dwp_flat = torch.zeros(total, dtype=F32, device=self.device)
         self._dwp, off = {}, 0
@@ -258,24 +277,27 @@ class Engine:
         rows = [(w, self._pack_buf("visual.cnn.conv1.weight", (64, 160)), 64 * 160, 64, 3, 7, 7, 160, 0),
                 (w, self._pack_buf("visual.cnn.conv1.weight#s2d", (64, 256)), 64 * 256, 64, 3, 7, 7, 256, 4)]
         for name, blk in self.blocks:
-            w = self.P(name + ".conv2.weight")
-            pl = w.shape[0]
-            rows.append((w, self._pack_buf(name + ".conv2.weight", (pl, 9 * pl)), 9 * pl * pl, pl, pl, 3, 3, 9 * pl, 0))
-            if blk.stride == 1:
-                rows.append((w, self._pack_buf(name + ".conv2.weight#dgrad", (pl, 9 * pl)), 9 * pl * pl, pl, pl, 3, 3,
-                             9 * pl, 1))
+            parity = []
+            for wname, stride in _convs3x3(name, blk):
+                w = self.P(wname + ".weight")
+                O, I = w.shape[0], w.shape[1]
+                rows.append((w, self._pack_buf(wname + ".weight", (O, 9 * I)), 9 * O * I, O, I, 3, 3, 9 * I, 0))
+                if stride == 1:
+                    rows.append((w, self._pack_buf(wname + ".weight#dgrad", (I, 9 * O)), 9 * O * I, O, I, 3, 3, 9 * O,
+                                 1))
+                else:  # stride-2 dgrad: one weight slice per parity class (ph, pw) of the input gradient
+                    for ph in (0, 1):
+                        for pw in (0, 1):
+                            nt = (1 + ph) * (1 + pw)
+                            parity.append((w, self._pack_buf(f"{wname}.weight#dgrad_s2_{ph}{pw}", (I, nt * O)),
+                                           nt * O * I, O, I, ph, pw, nt * O, 6))
             if blk.stride == 2 and blk.downsample is not None:
                 wdn = self.P(name + ".downsample.0.weight")
                 C4, Cin = wdn.shape[0], wdn.shape[1]
                 if Cin % 64 == 0:  # transposed copy: K-major B operand of the downsample's (implicit, strided-store) dgrad
                     rows.append((wdn, self._pack_buf(name + ".downsample.0.weight#t", (Cin, C4)), C4 * Cin, C4, Cin, 1, 1,
                                  C4, 7))
-            if blk.stride != 1:  # stride-2 dgrad: one weight slice per parity class (ph, pw) of the input gradient
-                for ph in (0, 1):
-                    for pw in (0, 1):
-                        nt = (1 + ph) * (1 + pw)
-                        rows.append((w, self._pack_buf(f"{name}.conv2.weight#dgrad_s2_{ph}{pw}", (pl, nt * pl)),
-                                     nt * pl * pl, pl, pl, ph, pw, nt * pl, 6))
+            rows += parity
         return rows
 
     def _unpack_rows(self, layer, stem_s2d):
@@ -285,10 +307,10 @@ class Engine:
         for name, blk in self.blocks:
             if name.split(".")[2] != want:
                 continue
-            pl = blk.conv2.weight.shape[0]
-            transposed = blk.stride == 1 and pl == 64  # halo-reuse wgrad writes [(tap, cin), cout]
-            rows.append((self._dwp[name + ".conv2"], self.G(name + ".conv2.weight"), 9 * pl * pl, pl, pl, 3, 3, 9 * pl,
-                         3 if transposed else 2))
+            for wname, stride in _convs3x3(name, blk):
+                O, I = self.G(wname + ".weight").shape[:2]
+                rows.append((self._dwp[wname], self.G(wname + ".weight"), 9 * O * I, O, I, 3, 3, 9 * I,
+                             3 if _transposed_wgrad(I, O, stride) else 2))
         if layer == "rest":
             g = self.G("visual.cnn.conv1.weight")
             if stem_s2d:
@@ -315,7 +337,9 @@ class Engine:
         out = [("visual.cnn.bn1", 64)]
         for name, blk in self.blocks:
             width, C4 = _block_widths(blk)
-            out += [(name + ".bn1", width), (name + ".bn2", width), (name + ".bn3", C4)]
+            out += [(name + ".bn1", width), (name + ".bn2", width)]
+            if not isinstance(blk, BasicBlock):
+                out.append((name + ".bn3", C4))
             if blk.downsample is not None:
                 out.append((name + ".downsample.1", C4))
         return out
@@ -353,7 +377,8 @@ class Engine:
         total = 2 * 64 * 2
         for name, blk in self.blocks:
             width, C4 = _block_widths(blk)
-            total += 2 * 2 * (width + width + C4 + (C4 if blk.downsample is not None else 0))
+            bn3 = 0 if isinstance(blk, BasicBlock) else C4
+            total += 2 * 2 * (width + width + bn3 + (C4 if blk.downsample is not None else 0))
         slab = self.ws.get("bn_slab", (total,), F32)
         slab.zero_()
         self._slab, self._slab_off = slab, 0
@@ -385,19 +410,19 @@ class Engine:
         gemm(cols, self._packed["visual.cnn.conv1.weight"], y0, M0, 64, 160, **epi)
         return None, cols
 
-    def _conv2(self, name, a1, y, B, Hc, Wc, stride, key, **epi):
-        """3x3 conv2 (stride) of block `name`: a1 [B*Hc*Wc, width] -> y [Mout, width]; returns the im2col matrix
-        when that route ran, else None."""
-        Mout, width = y.shape
-        w2 = self._packed[name + ".conv2.weight"]
-        if width % 64 == 0:
+    def _conv3x3(self, wname, x, y, B, Hc, Wc, stride, key, **epi):
+        """3x3 conv (stride 1 or 2, pad 1) whose weight is `wname`: x [B*Hc*Wc, Cin] -> y [Mout, C]; returns the
+        im2col matrix when that route ran, else None."""
+        Mout, C = y.shape
+        Cin = x.shape[1]
+        w = self._packed[wname + ".weight"]
+        if Cin % 64 == 0:
             # implicit GEMM: 4-D TMA boxes gather the taps (zero fill = padding); stride 2 through TMA traversal strides
-            gemm(a1, w2, y, Mout, width, 9 * width, lda=width, conv=(B, Hc, Wc, width), conv_mode=1,
-                 conv_stride=stride, **epi)
+            gemm(x, w, y, Mout, C, 9 * Cin, lda=Cin, conv=(B, Hc, Wc, Cin), conv_mode=1, conv_stride=stride, **epi)
             return None
-        cols = self.ws.get(key, (Mout, 9 * width), BF16)
-        call("vtx_im2col3x3", a1.data_ptr(), cols.data_ptr(), B, Hc, Wc, width, stride, _stream())
-        gemm(cols, w2, y, Mout, width, 9 * width, **epi)
+        cols = self.ws.get(key, (Mout, 9 * Cin), BF16)
+        call("vtx_im2col3x3", x.data_ptr(), cols.data_ptr(), B, Hc, Wc, Cin, stride, _stream())
+        gemm(cols, w, y, Mout, C, 9 * Cin, **epi)
         return cols
 
     def _downsample(self, name, x, y, B, Hc, Wc, stride, key, **epi):
@@ -419,8 +444,22 @@ class Engine:
         gemm(xs, wd, y, Mout, C4, Cin, **epi)
         return xs
 
+    def _block_output_fwd(self, rec, x, y, st, bn_name, out, mask, B, training):
+        """The last BN of block rec["name"] (input y, statistics st) + shortcut (x itself, or the downsample conv and
+        its BN) + ReLU into out, the ReLU sign bits into mask; returns the BN's bnp."""
+        name, Mout, C = rec["name"], rec["Mout"], rec["Cout"]
+        if rec["has_ds"]:
+            yd = self.ws.get(name + ".yd", (Mout, C), BF16)
+            std = self._slab_take(2 * C) if training else None
+            xs = self._downsample(name, x, yd, B, rec["Hin"], rec["Win"], rec["stride"], name + ".xs", stats=std)
+            bnpd = self._bn_fwd(yd, name + ".downsample.1", Mout, C, training, std)
+            rec.update(xs=xs, yd=yd, bnpd=bnpd)
+            return self._bn_act_fwd(y, bn_name, Mout, C, training, st, out, res=yd, bnp_res=bnpd, mask=mask)
+        return self._bn_act_fwd(y, bn_name, Mout, C, training, st, out, res=x, mask=mask)
+
     def backbone_forward(self, image: torch.Tensor, training: bool):
-        """image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, 2048]; fills the tape used by backward."""
+        """image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, C] (C = 2048 for the bottleneck ResNets, 512
+        for ResNet-18/34); fills the tape used by backward."""
         if not self._weights_fresh:
             self.prepare_weights()
         if training:
@@ -443,14 +482,31 @@ class Engine:
         call("vtx_bn_relu_maxpool", y0.data_ptr(), bnp0.data_ptr(), x.data_ptr(), idx.data_ptr(), B, Ho, Wo, 64, s)
         tape["stem"] = dict(cols=cols, s2d=s2d, y=y0, bnp=bnp0, idx=idx, Ho=Ho, Wo=Wo, Hp=Hp, Wp=Wp, M=M0)
         Hc, Wc, Cin = Hp, Wp, 64
-        # ---- bottleneck blocks
+        # ---- residual blocks
         for name, blk in self.blocks:
             width, C4 = _block_widths(blk)
             stride = blk.stride
             Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
             Min, Mout = B * Hc * Wc, B * Hn * Wn
             rec = dict(name=name, x=x, Hin=Hc, Win=Wc, Hout=Hn, Wout=Wn, Cin=Cin, width=width, Cout=C4, stride=stride,
-                       Min=Min, Mout=Mout, has_ds=blk.downsample is not None)
+                       Min=Min, Mout=Mout, has_ds=blk.downsample is not None, basic=isinstance(blk, BasicBlock))
+            if rec["basic"]:
+                # conv1 3x3 (stride) -> bn1 + ReLU -> conv2 3x3 -> bn2 + shortcut + ReLU (torchvision resnet.py:59-105)
+                y1 = ws.get(name + ".y1", (Mout, C4), BF16)
+                st1 = self._slab_take(2 * C4) if training else None
+                self._conv3x3(name + ".conv1", x, y1, B, Hc, Wc, stride, name + ".cols1", stats=st1)
+                a1 = ws.get(name + ".a1", (Mout, C4), BF16)
+                bnp1 = self._bn_act_fwd(y1, name + ".bn1", Mout, C4, training, st1, a1)
+                y2 = ws.get(name + ".y2", (Mout, C4), BF16)
+                st2 = self._slab_take(2 * C4) if training else None
+                self._conv3x3(name + ".conv2", a1, y2, B, Hn, Wn, 1, name + ".cols2", stats=st2)
+                out = ws.get(name + ".out", (Mout, C4), BF16)
+                m2 = ws.get(name + ".m2", (Mout, C4 // 8), torch.uint8) if training else None
+                bnp2 = self._block_output_fwd(rec, x, y2, st2, name + ".bn2", out, m2, B, training)
+                rec.update(y1=y1, bnp1=bnp1, a1=a1, y2=y2, bnp2=bnp2, out=out, m2=m2)
+                tape["blocks"].append(rec)
+                x, Hc, Wc, Cin = out, Hn, Wn, C4
+                continue
             # conv1 1x1
             y1 = ws.get(name + ".y1", (Min, width), BF16)
             st1 = self._slab_take(2 * width) if training else None
@@ -460,7 +516,7 @@ class Engine:
             # conv2 3x3 (stride)
             y2 = ws.get(name + ".y2", (Mout, width), BF16)
             st2 = self._slab_take(2 * width) if training else None
-            rec["cols2"] = self._conv2(name, a1, y2, B, Hc, Wc, stride, name + ".cols2", stats=st2)
+            rec["cols2"] = self._conv3x3(name + ".conv2", a1, y2, B, Hc, Wc, stride, name + ".cols2", stats=st2)
             a2 = ws.get(name + ".a2", (Mout, width), BF16)
             bnp2 = self._bn_act_fwd(y2, name + ".bn2", Mout, width, training, st2, a2)
             # conv3 1x1
@@ -471,15 +527,7 @@ class Engine:
             # backward needs only the SIGN of the block output's pre-activation: one bit per element instead of re-reading
             # the bf16 output twice (bn_bwd_reduce and bn_bwd_apply)
             m3 = ws.get(name + ".m3", (Mout, C4 // 8), torch.uint8) if training else None
-            if blk.downsample is not None:
-                yd = ws.get(name + ".yd", (Mout, C4), BF16)
-                std = self._slab_take(2 * C4) if training else None
-                xs = self._downsample(name, x, yd, B, Hc, Wc, stride, name + ".xs", stats=std)
-                bnpd = self._bn_fwd(yd, name + ".downsample.1", Mout, C4, training, std)
-                bnp3 = self._bn_act_fwd(y3, name + ".bn3", Mout, C4, training, st3, out, res=yd, bnp_res=bnpd, mask=m3)
-                rec.update(xs=xs, yd=yd, bnpd=bnpd)
-            else:
-                bnp3 = self._bn_act_fwd(y3, name + ".bn3", Mout, C4, training, st3, out, res=x, mask=m3)
+            bnp3 = self._block_output_fwd(rec, x, y3, st3, name + ".bn3", out, m3, B, training)
             rec.update(y1=y1, bnp1=bnp1, a1=a1, y2=y2, bnp2=bnp2, a2=a2, y3=y3, bnp3=bnp3, out=out, m3=m3)
             tape["blocks"].append(rec)
             x, Hc, Wc, Cin = out, Hn, Wn, C4
@@ -490,7 +538,7 @@ class Engine:
         return x, Hc, Wc
 
     def backbone_infer(self, image: torch.Tensor):
-        """Eval-mode backbone forward: image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, 2048].
+        """Eval-mode backbone forward: image fp32 NCHW [B,3,H,W] -> NHWC bf16 feature matrix [B*h*w, C].
         Every BN is the fixed per-channel affine map of its running statistics, applied by the epilogue of the GEMM
         that produces its input (VtxGemm.col_scale / col_shift), together with the shortcut and the ReLU: no raw conv
         output is stored and read back.  Writes no tape and no statistics; its buffers are its own, so a training
@@ -517,24 +565,34 @@ class Engine:
         call("vtx_bn_relu_maxpool", y0.data_ptr(), ws.flat["bnp_eval:visual.cnn.bn1"].data_ptr(), x.data_ptr(),
              idx.data_ptr(), B, Ho, Wo, 64, s)
         Hc, Wc, Cin = Hp, Wp, 64
-        # ---- bottleneck blocks: four GEMMs, each ending in its BN (+ shortcut) (+ ReLU); block outputs alternate
-        # between two buffers
+        # ---- residual blocks: each GEMM ends in its BN (+ shortcut) (+ ReLU), four per bottleneck, three per basic
+        # block with a downsample branch and two without; block outputs alternate between two buffers
         for bi, (name, blk) in enumerate(self.blocks):
             width, C4 = _block_widths(blk)
+            basic = isinstance(blk, BasicBlock)
             stride = blk.stride
             Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
             Min, Mout = B * Hc * Wc, B * Hn * Wn
-            a1 = ws.get("inf.a1", (Min, width), BF16)
-            gemm(x, self.W(name + ".conv1.weight").view(width, Cin), a1, Min, width, Cin, act=1, **ss(name + ".bn1"))
-            a2 = ws.get("inf.a2", (Mout, width), BF16)
-            self._conv2(name, a1, a2, B, Hc, Wc, stride, "inf.cols2", act=1, **ss(name + ".bn2"))
+            if basic:
+                a1 = ws.get("inf.a1", (Mout, width), BF16)
+                self._conv3x3(name + ".conv1", x, a1, B, Hc, Wc, stride, "inf.cols1", act=1, **ss(name + ".bn1"))
+            else:
+                a1 = ws.get("inf.a1", (Min, width), BF16)
+                gemm(x, self.W(name + ".conv1.weight").view(width, Cin), a1, Min, width, Cin, act=1,
+                     **ss(name + ".bn1"))
+                a2 = ws.get("inf.a2", (Mout, width), BF16)
+                self._conv3x3(name + ".conv2", a1, a2, B, Hc, Wc, stride, "inf.cols2", act=1, **ss(name + ".bn2"))
             shortcut = x
             if blk.downsample is not None:
                 shortcut = ws.get("inf.shortcut", (Mout, C4), BF16)
                 self._downsample(name, x, shortcut, B, Hc, Wc, stride, "inf.xs", **ss(name + ".downsample.1"))
             out = ws.get(f"inf.x{bi & 1}", (Mout, C4), BF16)
-            gemm(a2, self.W(name + ".conv3.weight").view(C4, width), out, Mout, C4, width, residual=shortcut, act=1,
-                 **ss(name + ".bn3"))
+            if basic:
+                self._conv3x3(name + ".conv2", a1, out, B, Hn, Wn, 1, "inf.cols2", residual=shortcut, act=1,
+                              **ss(name + ".bn2"))
+            else:
+                gemm(a2, self.W(name + ".conv3.weight").view(C4, width), out, Mout, C4, width, residual=shortcut,
+                     act=1, **ss(name + ".bn3"))
             x, Hc, Wc, Cin = out, Hn, Wn, C4
         return x, Hc, Wc
 
@@ -571,6 +629,70 @@ class Engine:
                  y.data_ptr(), bnp.data_ptr(), dy.data_ptr(), y2.data_ptr(), bnp2.data_ptr(), dy2.data_ptr(),
                  _p(dz_out), M, C, mask_from_y, s)
 
+    def _wgrad3x3(self, dy, x, dwp, B, Hc, Wc, stride):
+        """Weight gradient of a 3x3 conv (stride) into its fp32 scratch dwp [C, 9 * Cin] (fp32 atomics): dy [Mout, C],
+        x [B*Hc*Wc, Cin], both read in place by implicit GEMMs."""
+        Mout, C = dy.shape
+        Cin = x.shape[1]
+        if _transposed_wgrad(Cin, C, stride):
+            # wgrad in the [(tap, cin), cout] layout (vtx_conv_w_unpack_add_t folds it into OIHW)
+            gemm(dy, x, dwp, 9 * Cin, C, Mout, atomic=True, lda=C, ldb=Cin, ldd=C, conv=(B, Hc, Wc, Cin), conv_mode=4,
+                 out_f32=True)
+        else:
+            tiles = ((C + 127) // 128) * ((9 * Cin + 255) // 256)
+            sk = ops.split_k_for(tiles, (Mout + 63) // 64)
+            gemm(dy, x, dwp, C, 9 * Cin, Mout, atomic=True, split_k=sk, lda=C, ldb=Cin, conv=(B, Hc, Wc, Cin),
+                 conv_mode=2, out_f32=True, conv_stride=stride)
+
+    def _dgrad3x3_s2(self, dy, wname, dx, B, Hc, Wc, bnr=None):
+        """Input gradient dx [B*Hc*Wc, Cin] of a stride-2 3x3 conv from dy [Mout, C] as four implicit GEMMs, one per
+        parity class (ph, pw) of the input position: row 2i+ph of dx gathers dy rows i+a, a < 1+ph, through kernel rows
+        ph+1-2a (same along w); each class writes its own strided sub-grid of dx, so every element is written exactly
+        once -- no per-tap gradient matrix, no col2im scatter.  bnr = (y, bnp, sums): the BN-backward sums of the BN
+        whose output gradient dx is, accumulated by the epilogues (ReLU mask recomputed from y)."""
+        Mout, C = dy.shape
+        Cin = dx.shape[1]
+        Hn, Wn = (Hc - 1) // 2 + 1, (Wc - 1) // 2 + 1
+        for ph in (0, 1):
+            for pw in (0, 1):
+                th, tw = 1 + ph, 1 + pw
+                Hs, Ws = (Hc - ph + 1) // 2, (Wc - pw + 1) // 2
+                if Hs <= 0 or Ws <= 0:
+                    continue
+                voff = (ph * Wc + pw) * Cin * 2
+                epi = {} if bnr is None else dict(bnr=(bnr[0], bnr[1], bnr[2], None, bnr[0].data_ptr() + voff))
+                gemm(dy, self._packed[f"{wname}.weight#dgrad_s2_{ph}{pw}"], dx, Mout, Cin, th * tw * C, lda=C,
+                     conv=(B, Hn, Wn, C), conv_mode=1, tap_grid=(th, tw, 0), d_ptr=dx.data_ptr() + voff,
+                     out_view=(Hs, Ws, 2 * Cin, 2 * Wc * Cin, Hc * Wc * Cin), **epi)
+
+    def _downsample_wgrad(self, rec, dyd, B):
+        """Weight gradient of block rec's 1x1 shortcut conv from its output gradient dyd [Mout, C4]."""
+        name, Mout, C4, Cin = rec["name"], rec["Mout"], rec["Cout"], rec["Cin"]
+        if rec["xs"] is not None:
+            self._wgrad(dyd, rec["xs"], self.G(name + ".downsample.0.weight"), C4, Cin, Mout)
+        else:  # one-tap implicit wgrad over the strided view of x, straight into the [C4, Cin, 1, 1] gradient
+            tiles = ((C4 + 127) // 128) * ((Cin + 255) // 256)
+            gemm(dyd, rec["x"], self.G(name + ".downsample.0.weight").view(C4, Cin), C4, Cin, Mout, atomic=True,
+                 split_k=ops.split_k_for(tiles, (Mout + 63) // 64), lda=C4, ldb=Cin, conv=(B, rec["Hin"], rec["Win"], Cin),
+                 conv_mode=2, conv_stride=rec["stride"], conv_taps=1, out_f32=True)
+
+    def _downsample_dgrad_add(self, rec, dyd, dx, B):
+        """dx [Min, Cin] += the input gradient of block rec's 1x1 shortcut conv, from dyd [Mout, C4]."""
+        name, Min, Mout, C4, Cin, stride = rec["name"], rec["Min"], rec["Mout"], rec["Cout"], rec["Cin"], rec["stride"]
+        Hc, Wc = rec["Hin"], rec["Win"]
+        if stride == 1:
+            gemm(dyd, self.W(name + ".downsample.0.weight").view(C4, Cin), dx, Min, Cin, C4, b_mn=1, residual=dx)
+        elif stride == 2 and rec["xs"] is None:
+            # dx[:, ::2, ::2] += dyd . Wd: one-tap implicit GEMM over the dyd grid whose output (and residual) is
+            # the even-position sub-grid of dx -- in-place accumulation, no dxs buffer, no upsample_add pass
+            gemm(dyd, self._packed[name + ".downsample.0.weight#t"], dx, Mout, Cin, C4, lda=C4,
+                 conv=(B, rec["Hout"], rec["Wout"], C4), conv_mode=1, conv_taps=1, residual=dx, d_ptr=dx.data_ptr(),
+                 out_view=((Hc + 1) // 2, (Wc + 1) // 2, 2 * Cin, 2 * Wc * Cin, Hc * Wc * Cin))
+        else:
+            dxs = self.ws.get("bwd.dxs", (Mout, Cin), BF16)
+            gemm(dyd, self.W(name + ".downsample.0.weight").view(C4, Cin), dxs, Mout, Cin, C4, b_mn=1)
+            call("vtx_upsample_add", dxs.data_ptr(), dx.data_ptr(), B, Hc, Wc, Cin, stride, _stream())
+
     def backbone_backward(self, dfeat: torch.Tensor, bucket_cb=None):
         """dfeat bf16 [B*h*w, C]: gradient w.r.t. the backbone output.  Accumulates into the gradient arena.
         `bucket_cb(tag)` is called when every gradient of 'layer4' / 'layer3' / 'layer2' has been enqueued."""
@@ -600,6 +722,11 @@ class Engine:
             prev_layer = layer
             Min, Mout, C4 = rec["Min"], rec["Mout"], rec["Cout"]
             Hc, Wc, Hn, Wn = rec["Hin"], rec["Win"], rec["Hout"], rec["Wout"]
+            if rec["basic"]:
+                dOut, sums3 = self._basic_block_bwd(rec, blocks[bi - 1] if bi > 0 else None, dOut, sums3,
+                                                    ws.get(f"bwd.dx{scratch_i & 1}", (Min, Cin), BF16), B)
+                scratch_i += 1
+                continue
             # ---- block output: ReLU mask + bn3 (+ downsample BN) backward
             dy3 = ws.get("bwd.dy3", (Mout, C4), BF16)
             if rec["has_ds"]:
@@ -627,37 +754,14 @@ class Engine:
             da1 = ws.get("bwd.da1", (Min, width), BF16)
             sums1 = None
             if rec["cols2"] is None:
-                if width == 64 and stride == 1:
-                    # wgrad in the [(tap, cin), cout] layout (vtx_conv_w_unpack_add_t folds it into OIHW)
-                    gemm(dy2, rec["a1"], dwp, 9 * width, width, Mout, atomic=True, lda=width, ldb=width, ldd=width,
-                         conv=(B, Hc, Wc, width), conv_mode=4, out_f32=True)
-                else:
-                    tiles = ((width + 127) // 128) * ((9 * width + 255) // 256)
-                    sk = ops.split_k_for(tiles, (Mout + 63) // 64)
-                    gemm(dy2, rec["a1"], dwp, width, 9 * width, Mout, atomic=True, split_k=sk, lda=width,
-                         ldb=width, conv=(B, Hc, Wc, width), conv_mode=2, out_f32=True, conv_stride=stride)
+                self._wgrad3x3(dy2, rec["a1"], dwp, B, Hc, Wc, stride)
                 if stride in (1, 2):
                     sums1 = self._slab_take(2 * width)  # bn1's backward sums, accumulated by the conv2-dgrad epilogue(s)
                 if stride == 1:
                     gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Min, width, 9 * width, lda=width,
                          conv=(B, Hc, Wc, width), conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
                 elif stride == 2:
-                    # strided dgrad as four implicit GEMMs, one per parity class (ph, pw) of the input position: row
-                    # 2i+ph of da1 gathers dy rows i+a, a < 1+ph, through kernel rows ph+1-2a (same along w); each class
-                    # writes its own strided sub-grid of da1, so every element is written exactly once -- no per-tap
-                    # gradient matrix, no col2im scatter
-                    for ph in (0, 1):
-                        for pw in (0, 1):
-                            th, tw = 1 + ph, 1 + pw
-                            Hs, Ws = (Hc - ph + 1) // 2, (Wc - pw + 1) // 2
-                            if Hs <= 0 or Ws <= 0:
-                                continue
-                            voff = (ph * Wc + pw) * width * 2
-                            gemm(dy2, self._packed[f"{name}.conv2.weight#dgrad_s2_{ph}{pw}"], da1, Mout, width,
-                                 th * tw * width, lda=width, conv=(B, Hn, Wn, width), conv_mode=1, tap_grid=(th, tw, 0),
-                                 d_ptr=da1.data_ptr() + voff,
-                                 out_view=(Hs, Ws, 2 * width, 2 * Wc * width, Hc * Wc * width),
-                                 bnr=(rec["y1"], rec["bnp1"], sums1, None, rec["y1"].data_ptr() + voff))
+                    self._dgrad3x3_s2(dy2, name + ".conv2", da1, B, Hc, Wc, bnr=(rec["y1"], rec["bnp1"], sums1))
                 else:  # other strides: per-tap gradients by a plain GEMM, scattered back by col2im
                     dcols = ws.get("bwd.dcols", (Mout, 9 * width), BF16)
                     gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * width, width, b_mn=1)
@@ -676,27 +780,9 @@ class Engine:
             scratch_i += 1
             w1 = self.W(name + ".conv1.weight").view(width, Cin)
             if rec["has_ds"]:
-                wd = self.W(name + ".downsample.0.weight").view(C4, Cin)
-                if rec["xs"] is not None:
-                    self._wgrad(dyd, rec["xs"], self.G(name + ".downsample.0.weight"), C4, Cin, Mout)
-                else:  # one-tap implicit wgrad over the strided view of x, straight into the [C4, Cin, 1, 1] gradient
-                    tiles = ((C4 + 127) // 128) * ((Cin + 255) // 256)
-                    gemm(dyd, rec["x"], self.G(name + ".downsample.0.weight").view(C4, Cin), C4, Cin, Mout, atomic=True,
-                         split_k=ops.split_k_for(tiles, (Mout + 63) // 64), lda=C4, ldb=Cin, conv=(B, Hc, Wc, Cin),
-                         conv_mode=2, conv_stride=stride, conv_taps=1, out_f32=True)
+                self._downsample_wgrad(rec, dyd, B)
                 gemm(dy1, w1, dx, Min, Cin, width, b_mn=1)
-                if stride == 1:
-                    gemm(dyd, wd, dx, Min, Cin, C4, b_mn=1, residual=dx)
-                elif stride == 2 and rec["xs"] is None:
-                    # dx[:, ::2, ::2] += dyd . Wd: one-tap implicit GEMM over the dyd grid whose output (and residual) is
-                    # the even-position sub-grid of dx -- in-place accumulation, no dxs buffer, no upsample_add pass
-                    gemm(dyd, self._packed[name + ".downsample.0.weight#t"], dx, Mout, Cin, C4, lda=C4,
-                         conv=(B, Hn, Wn, C4), conv_mode=1, conv_taps=1, residual=dx, d_ptr=dx.data_ptr(),
-                         out_view=((Hc + 1) // 2, (Wc + 1) // 2, 2 * Cin, 2 * Wc * Cin, Hc * Wc * Cin))
-                else:
-                    dxs = ws.get("bwd.dxs", (Mout, Cin), BF16)
-                    gemm(dyd, wd, dxs, Mout, Cin, C4, b_mn=1)
-                    call("vtx_upsample_add", dxs.data_ptr(), dx.data_ptr(), B, Hc, Wc, Cin, stride, s)
+                self._downsample_dgrad_add(rec, dyd, dx, B)
             else:
                 # dx is the output gradient of the previous block: when that block has a single-branch bn3, its backward
                 # sums (ReLU bit mask m3 of THAT block) are accumulated here, over the staged dx tiles
@@ -723,6 +809,53 @@ class Engine:
             self._wgrad(dy0, st["cols"], dwp0, 64, 160, M0)
         # layer1's 3x3 weight gradients + the stem's, in one launch (the 'rest' all-reduce bucket follows)
         self._run_jobs("unpack:rest:" + ("s2d" if stem_s2d else "cols"), lambda: self._unpack_rows("rest", stem_s2d))
+
+    def _basic_block_bwd(self, rec, prev, dOut, sums2, dx, B):
+        """Backward of one basic block from its output gradient dOut into dx [Min, Cin], its parameter gradients
+        accumulated; `sums2`: bn2's backward sums when the GEMM that produced dOut already accumulated them.  Returns
+        (dx, the previous block's bn2 sums when this block's conv1 dgrad accumulated them, else None)."""
+        ws = self.ws
+        name, Cin, C, stride = rec["name"], rec["Cin"], rec["Cout"], rec["stride"]
+        Min, Mout, Hn, Wn = rec["Min"], rec["Mout"], rec["Hout"], rec["Wout"]
+        # ---- block output: ReLU mask + bn2 (+ downsample BN) backward
+        dy2 = ws.get("bwd.dy2", (Mout, C), BF16)
+        dyd = None
+        if rec["has_ds"]:
+            dyd = ws.get("bwd.dyd", (Mout, C), BF16)
+            self._bn_bwd(dOut, rec["m2"], rec["y2"], rec["bnp2"], name + ".bn2", Mout, C, dy2,
+                         two=(rec["yd"], rec["bnpd"], name + ".downsample.1", dyd))
+        else:
+            self._bn_bwd(dOut, rec["m2"], rec["y2"], rec["bnp2"], name + ".bn2", Mout, C, dy2, sums=sums2)
+        # ---- conv2 (3x3, stride 1): wgrad + dgrad; the dgrad epilogue accumulates bn1's sums (ReLU mask from y1)
+        self._wgrad3x3(dy2, rec["a1"], self._dwp[name + ".conv2"].view(C, 9 * C), B, Hn, Wn, 1)
+        da1 = ws.get("bwd.da1", (Mout, C), BF16)
+        sums1 = self._slab_take(2 * C)
+        gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Mout, C, 9 * C, lda=C, conv=(B, Hn, Wn, C),
+             conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
+        dy1 = ws.get("bwd.dy1", (Mout, C), BF16)
+        self._bn_bwd(da1, None, rec["y1"], rec["bnp1"], name + ".bn1", Mout, C, dy1, mask_from_y=1, sums=sums1)
+        # ---- conv1 (3x3, stride): wgrad + dgrad (+ shortcut gradient)
+        Hc, Wc = rec["Hin"], rec["Win"]
+        self._wgrad3x3(dy1, rec["x"], self._dwp[name + ".conv1"].view(C, 9 * Cin), B, Hc, Wc, stride)
+        if rec["has_ds"]:
+            self._downsample_wgrad(rec, dyd, B)
+            if stride == 2:
+                self._dgrad3x3_s2(dy1, name + ".conv1", dx, B, Hc, Wc)
+            else:
+                gemm(dy1, self._packed[name + ".conv1.weight#dgrad"], dx, Min, Cin, 9 * C, lda=C, conv=(B, Hc, Wc, C),
+                     conv_mode=1)
+            self._downsample_dgrad_add(rec, dyd, dx, B)
+            return dx, None
+        # identity block: the shortcut gradient dOut * [block output > 0] is never written -- conv1's dgrad epilogue
+        # adds dOut under the block's bit mask; dx is the output gradient of the previous block, whose bn2 sums (under
+        # THAT block's bit mask) the same epilogue accumulates when the previous block has a single-branch bn2
+        bnr, sums_prev = None, None
+        if prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
+            sums_prev = self._slab_take(2 * Cin)
+            bnr = (prev["y2"], prev["bnp2"], sums_prev, prev["m2"])
+        gemm(dy1, self._packed[name + ".conv1.weight#dgrad"], dx, Min, Cin, 9 * C, lda=C, conv=(B, Hc, Wc, C),
+             conv_mode=1, residual=dOut, residual_mask=rec["m2"], bnr=bnr)
+        return dx, sums_prev
 
     # ------------------------------------------------------------------------------------------------ head
     def _head_modules(self, direction):

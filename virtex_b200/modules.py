@@ -13,10 +13,14 @@ from typing import List, Optional
 import torch
 from torch import nn
 
-# torchvision ResNet name -> (bottleneck blocks per layer, width_per_group).  A bottleneck of `planes` has inner width
-# planes * width_per_group / 64 and output width 4 * planes (torchvision/models/resnet.py:108-163, groups = 1).
-_RESNET_ARCHS = {"resnet50": ([3, 4, 6, 3], 64), "resnet101": ([3, 4, 23, 3], 64), "resnet152": ([3, 8, 36, 3], 64),
-                 "wide_resnet50_2": ([3, 4, 6, 3], 128), "wide_resnet101_2": ([3, 4, 23, 3], 128)}
+# torchvision ResNet name -> (blocks per layer, width_per_group, block kind).  A bottleneck of `planes` has inner width
+# planes * width_per_group / 64 and output width 4 * planes (torchvision/models/resnet.py:108-163, groups = 1); a basic
+# block of `planes` is two 3x3 convs of width `planes` (resnet.py:59-105).
+_RESNET_ARCHS = {"resnet18": ([2, 2, 2, 2], 64, "basic"), "resnet34": ([3, 4, 6, 3], 64, "basic"),
+                 "resnet50": ([3, 4, 6, 3], 64, "bottleneck"), "resnet101": ([3, 4, 23, 3], 64, "bottleneck"),
+                 "resnet152": ([3, 8, 36, 3], 64, "bottleneck"),
+                 "wide_resnet50_2": ([3, 4, 6, 3], 128, "bottleneck"),
+                 "wide_resnet101_2": ([3, 4, 23, 3], 128, "bottleneck")}
 
 
 class _NoForward(nn.Module):
@@ -46,12 +50,31 @@ class Bottleneck(_NoForward):
                                             nn.BatchNorm2d(planes * 4))
 
 
+class BasicBlock(_NoForward):
+    """Parameters of torchvision's BasicBlock (torchvision/models/resnet.py:59-105): 3x3(stride) -> 3x3, both of width
+    `planes`; the shortcut is a strided 1x1 conv + BN where the stride or the width changes."""
+    expansion = 1
+
+    def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: bool = False):
+        super().__init__()
+        self.conv1 = nn.Conv2d(inplanes, planes, 3, stride=stride, padding=1, bias=False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = nn.Conv2d(planes, planes, 3, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.stride = stride
+        self.downsample = None
+        if downsample:
+            self.downsample = nn.Sequential(nn.Conv2d(inplanes, planes, 1, stride=stride, bias=False),
+                                            nn.BatchNorm2d(planes))
+
+
 class ResNetParams(_NoForward):
-    """Parameter tree of torchvision ResNet-50/101/152 and Wide ResNet-50-2/101-2 up to layer4 (`fc` replaced by
-    Identity as in the reference).  Every one ends in 2048 channels.
+    """Parameter tree of torchvision ResNet-18/34/50/101/152 and Wide ResNet-50-2/101-2 up to layer4 (`fc` replaced by
+    Identity as in the reference).  ResNet-18/34 (basic blocks) end in 512 channels, the bottleneck ResNets in 2048
+    (`out_channels`).
 
     Callable like torchvision's ResNet (the downstream evaluations, scripts/clf_linear.py and scripts/clf_voc07.py):
-    `forward(image fp32 (B,3,H,W)) -> fc(flatten(avgpool(layer4)))` in fp32, the (B, 2048) pooled features while `fc`
+    `forward(image fp32 (B,3,H,W)) -> fc(flatten(avgpool(layer4)))` in fp32, the (B, out_channels) pooled features while `fc`
     is nn.Identity, logits once an nn.Linear is assigned to `fc`.  In eval mode every BatchNorm uses its running
     statistics, folded into the GEMM epilogues (Engine.backbone_infer), and gradients reach `fc` only; the backbone
     must then be frozen (requires_grad False) or the call made under no_grad.  In train mode BN uses batch statistics
@@ -61,8 +84,10 @@ class ResNetParams(_NoForward):
         super().__init__()
         if name not in _RESNET_ARCHS:
             raise KeyError(f"unsupported torchvision backbone '{name}' (supported: {sorted(_RESNET_ARCHS)})")
-        blocks_per_layer, width_per_group = _RESNET_ARCHS[name]
+        blocks_per_layer, width_per_group, kind = _RESNET_ARCHS[name]
         self.blocks_per_layer: List[int] = list(blocks_per_layer)
+        expansion = 1 if kind == "basic" else 4
+        self.out_channels = 512 * expansion
         self.conv1 = nn.Conv2d(3, 64, 7, stride=2, padding=3, bias=False)
         self.bn1 = nn.BatchNorm2d(64)
         inplanes = 64
@@ -70,9 +95,13 @@ class ResNetParams(_NoForward):
             blocks = []
             for bi in range(n):
                 stride = 2 if (bi == 0 and li > 1) else 1
-                blocks.append(Bottleneck(inplanes, planes, stride, downsample=(stride != 1 or inplanes != planes * 4),
-                                         width=planes * width_per_group // 64))
-                inplanes = planes * 4
+                downsample = stride != 1 or inplanes != planes * expansion
+                if kind == "basic":
+                    blocks.append(BasicBlock(inplanes, planes, stride, downsample=downsample))
+                else:
+                    blocks.append(Bottleneck(inplanes, planes, stride, downsample=downsample,
+                                             width=planes * width_per_group // 64))
+                inplanes = planes * expansion
             setattr(self, f"layer{li}", nn.Sequential(*blocks))
         self.avgpool = nn.AdaptiveAvgPool2d((1, 1))  # torchvision's attribute (no state); forward pools in CUDA
         self.fc = nn.Identity()
@@ -87,6 +116,8 @@ class ResNetParams(_NoForward):
             for m in self.modules():
                 if isinstance(m, Bottleneck):
                     nn.init.constant_(m.bn3.weight, 0)
+                elif isinstance(m, BasicBlock):
+                    nn.init.constant_(m.bn2.weight, 0)
 
     def forward(self, image: torch.Tensor) -> torch.Tensor:
         from .engine import resnet_forward
@@ -115,6 +146,9 @@ class TorchvisionVisualBackbone(VisualBackbone):
         if pretrained:
             raise RuntimeError("pretrained torchvision weights need a download; load a state_dict instead (no network)")
         self.cnn = ResNetParams(name, zero_init_residual=True)
+        if self.cnn.out_channels == 512 and visual_feature_size != 512:
+            raise ValueError(f"torchvision backbone '{name}' outputs 512 channels: set MODEL.VISUAL.FEATURE_SIZE 512 "
+                             f"(got visual_feature_size={visual_feature_size})")
         self.frozen = frozen
         if frozen:
             for p in self.cnn.parameters():
