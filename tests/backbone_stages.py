@@ -13,7 +13,7 @@ reference and sum_k |a_k b_k| of each element (`mag`); a bound is built from the
   * BN apply, ReLU bit mask, max pool: bit-exact through the replicas of tests/backbone_replica.py.
 
 `exact=True` replaces each replica by plain float64 arithmetic: chained that way, the stages reproduce float64 autograd
-of torchvision's Bottleneck and of the stem.
+of torchvision's Bottleneck, of its BasicBlock and of the stem.
 """
 import math
 
@@ -185,6 +185,43 @@ def block_dx(dy1, w1, H, W, dOut=None, keep3=None, dyd=None, wd=None, stride=1):
     E2 = gemm_err(m2, dyd.shape[-1])
     ref = t1 + t2
     return ref, bf16_bound(ref, E1 + E2, t1, t2)
+
+
+def _dgrad_err(mag, C, stride):
+    """E of a 3x3 / pad 1 conv dgrad of C output channels: one 9-tap launch at stride 1; at stride 2 one launch per
+    parity class (ph, pw) of the input position, (1 + ph) * (1 + pw) taps long."""
+    if stride == 1:
+        return gemm_err(mag, 9 * C)
+    E = mag.new_empty(mag.shape)
+    for ph in (0, 1):
+        for pw in (0, 1):
+            E[:, ph::2, pw::2] = gemm_err(mag[:, ph::2, pw::2], (1 + ph) * (1 + pw) * C)
+    return E
+
+
+def basic_block_dx(dy1, w1, stride, H, W, dOut=None, keep2=None, dyd=None, wd=None):
+    """Outgoing gradient [N, H, W, Cin] of a basic block and its bound: the 3x3 conv1 dgrad dy1 . W1 (stride) plus the
+    shortcut term.
+
+    Identity block: dOut * keep2, added by the dgrad's own epilogue (residual under the bit mask) to its
+    bf16-rounded tile, so E carries |dOut * keep2| and the bound one more ulp of the dgrad.  Transition block: dyd . Wd
+    at the stride positions, a second launch that reads the stored conv1 dgrad (bf16) as its residual and adds it to
+    its own bf16-rounded tile: three roundings and both accumulations where it lands, the conv1 dgrad's alone
+    elsewhere (the odd positions of a stride-2 block)."""
+    t1, m1 = conv_dgrad(dy1, w1, stride, 1, H, W)
+    E1 = _dgrad_err(m1, dy1.shape[-1], stride)
+    if wd is None:
+        sc = dOut * keep2
+        ref = t1 + sc
+        return ref, bf16_bound(ref, E1 + gemm_err(sc.abs(), 9 * dy1.shape[-1]), t1)
+    t2, m2 = conv_dgrad(dyd, wd, stride, 0, H, W)
+    stored = t1.abs() + E1 + R.ulp_bf16(t1.abs() + E1)  # |the bf16 conv1 dgrad| the second launch reads
+    on = torch.zeros_like(t1[..., :1])
+    on[:, ::stride, ::stride] = 1.0
+    E = E1 + on * gemm_err(m2 + stored, dyd.shape[-1])
+    ref = t1 + t2
+    b = E + R.ulp_bf16(ref.abs() + E)
+    return ref, b + on * (R.ulp_bf16(t1.abs() + E1) + R.ulp_bf16(t2.abs() + E))
 
 
 def maxpool_backward(dpool, idx, H, W):

@@ -1,11 +1,11 @@
 """The stage references of tests/backbone_stages.py, fed exact float64 values and chained with no rounding in between,
-against float64 autograd of torchvision's Bottleneck and of the ResNet stem (7x7 / stride 2 conv, train-mode BN, ReLU,
-3x3 / stride 2 max pool): every forward value, every intermediate gradient, every weight and BN parameter gradient
-(biases included) and the outgoing input gradient, to 1e-12 relative to the largest value of each."""
+against float64 autograd of torchvision's Bottleneck, of its BasicBlock and of the ResNet stem (7x7 / stride 2 conv,
+train-mode BN, ReLU, 3x3 / stride 2 max pool): every forward value, every intermediate gradient, every weight and BN
+parameter gradient (biases included) and the outgoing input gradient, to 1e-12 relative to the largest value of each."""
 import pytest
 import torch
 from torch import nn
-from torchvision.models.resnet import Bottleneck
+from torchvision.models.resnet import BasicBlock, Bottleneck
 
 from tests import backbone_replica as R
 from tests import backbone_stages as S
@@ -147,6 +147,94 @@ def test_bottleneck_stages_match_autograd(Cin, planes, stride, H, W):
     _close(S.conv_wgrad(dy3, a2, 1, 1, 1, 0)[0], blk.conv3.weight.grad, "conv3 dW")
     _close(S.conv_wgrad(dy2, a1, 3, 3, stride, 1)[0], blk.conv2.weight.grad, "conv2 dW")
     _close(S.conv_wgrad(dy1, xh, 1, 1, 1, 0)[0], blk.conv1.weight.grad, "conv1 dW")
+    if down is not None:
+        _close(S.conv_wgrad(dyd, xh, 1, 1, stride, 0)[0], down[0].weight.grad, "downsample.0 dW")
+
+
+BASIC_BLOCKS = [  # (Cin, planes, stride, H, W): identity, stride-2 transition on an odd extent, stride-1 Cin != C
+    pytest.param(16, 16, 1, 9, 11, id="identity"),
+    pytest.param(8, 16, 2, 13, 15, id="transition-s2-13x15"),
+    pytest.param(8, 16, 1, 8, 6, id="transition-s1"),
+]
+
+
+@pytest.mark.parametrize("Cin,planes,stride,H,W", BASIC_BLOCKS)
+def test_basic_block_stages_match_autograd(Cin, planes, stride, H, W):
+    g = torch.Generator().manual_seed(7 * Cin + planes + H * W)
+    torch.manual_seed(Cin * stride + W)
+    C = planes
+    down = None
+    if stride != 1 or Cin != C:
+        down = nn.Sequential(nn.Conv2d(Cin, C, 1, stride=stride, bias=False), nn.BatchNorm2d(C))
+    blk = BasicBlock(Cin, planes, stride=stride, downsample=down).to(F64).train()
+    blk.relu = nn.ReLU()  # the shared in-place ReLU would overwrite the BN outputs the hooks keep
+    for bn in [blk.bn1, blk.bn2] + ([down[1]] if down is not None else []):
+        _live_bn(bn, g)
+    N = 3
+    x = torch.randn(N, Cin, H, W, generator=g, dtype=F64).requires_grad_(True)
+    mods = {"conv1": blk.conv1, "conv2": blk.conv2}
+    if down is not None:
+        mods["ds"] = down[0]
+    seen = _capture(mods)
+    out = blk(x)
+    dOut = torch.randn(out.shape, generator=g, dtype=F64)
+    out.backward(dOut)
+
+    w = {k: m.weight.detach() for k, m in mods.items()}
+    xh = _nhwc(x.detach())
+    Ho, Wo = S.out_extent(H, W, 3, stride, 1)
+    Mout = N * Ho * Wo
+    # ---- forward
+    y1 = S.conv(xh, w["conv1"], stride, 1)[0]
+    _close(y1, _nhwc(seen["conv1"][1]), "y1")
+    bnp1 = S.bn_params(y1.reshape(Mout, -1), blk.bn1.weight.detach(), blk.bn1.bias.detach())
+    a1 = S.bn_apply(y1.reshape(Mout, -1), bnp1, exact=True)[1].view(N, Ho, Wo, -1)
+    _close(a1, _nhwc(seen["conv2"][0]), "a1")
+    y2 = S.conv(a1, w["conv2"], 1, 1)[0]
+    _close(y2, _nhwc(seen["conv2"][1]), "y2")
+    bnp2 = S.bn_params(y2.reshape(Mout, -1), blk.bn2.weight.detach(), blk.bn2.bias.detach())
+    if down is not None:
+        yd = S.conv(xh, w["ds"], stride, 0)[0]
+        _close(yd, _nhwc(seen["ds"][1]), "yd")
+        bnpd = S.bn_params(yd.reshape(Mout, -1), down[1].weight.detach(), down[1].bias.detach())
+        pre2, o = S.bn_apply(y2.reshape(Mout, -1), bnp2, res=yd.reshape(Mout, -1), bnp_res=bnpd, exact=True)
+    else:
+        pre2, o = S.bn_apply(y2.reshape(Mout, -1), bnp2, res=xh.reshape(Mout, -1), exact=True)
+    _close(o.view(N, Ho, Wo, -1), _nhwc(out), "block output")
+    assert torch.equal(R.unpack_mask(R.pack_mask(pre2 > 0), C), pre2 > 0)
+    # ---- backward
+    dO = _nhwc(dOut).reshape(Mout, C)
+    dz2 = dO * (pre2 > 0)
+    sums2 = S.bn_sums(dz2, y2.reshape(Mout, -1), bnp2)[0]
+    dy2 = S.bn_backward(dO, pre2 > 0, y2.reshape(Mout, -1), bnp2, sums2, Mout)[1].view(N, Ho, Wo, -1)
+    _close(dy2, _nhwc(seen["conv2"][1].grad), "dy2")
+    _close(sums2[1], blk.bn2.weight.grad, "bn2 dgamma")
+    _close(sums2[0], blk.bn2.bias.grad, "bn2 dbeta")
+    dyd = None
+    if down is not None:
+        sumsd = S.bn_sums(dz2, yd.reshape(Mout, -1), bnpd)[0]
+        dyd = S.bn_backward(dO, pre2 > 0, yd.reshape(Mout, -1), bnpd, sumsd, Mout)[1].view(N, Ho, Wo, -1)
+        _close(dyd, _nhwc(seen["ds"][1].grad), "dyd")
+        _close(sumsd[1], down[1].weight.grad, "downsample.1 dgamma")
+        _close(sumsd[0], down[1].bias.grad, "downsample.1 dbeta")
+    da1 = S.conv_dgrad(dy2, w["conv2"], 1, 1, Ho, Wo)[0]
+    _close(da1, _nhwc(seen["conv2"][0].grad), "da1")
+    keep1 = S.relu_keep(y1.reshape(Mout, -1), bnp1, exact=True)
+    sums1 = S.bn_sums(da1.reshape(Mout, -1) * keep1, y1.reshape(Mout, -1), bnp1)[0]
+    dy1 = S.bn_backward(da1.reshape(Mout, -1), keep1, y1.reshape(Mout, -1), bnp1, sums1, Mout)[1]
+    dy1 = dy1.view(N, Ho, Wo, -1)
+    _close(dy1, _nhwc(seen["conv1"][1].grad), "dy1")
+    _close(sums1[1], blk.bn1.weight.grad, "bn1 dgamma")
+    _close(sums1[0], blk.bn1.bias.grad, "bn1 dbeta")
+    if down is None:
+        dx = S.basic_block_dx(dy1, w["conv1"], stride, H, W, dOut=_nhwc(dOut),
+                              keep2=(pre2 > 0).view(N, Ho, Wo, -1))[0]
+    else:
+        dx = S.basic_block_dx(dy1, w["conv1"], stride, H, W, dyd=dyd, wd=w["ds"])[0]
+    _close(dx, _nhwc(x.grad), "dx")
+    # ---- weight gradients
+    _close(S.conv_wgrad(dy2, a1, 3, 3, 1, 1)[0], blk.conv2.weight.grad, "conv2 dW")
+    _close(S.conv_wgrad(dy1, xh, 3, 3, stride, 1)[0], blk.conv1.weight.grad, "conv1 dW")
     if down is not None:
         _close(S.conv_wgrad(dyd, xh, 1, 1, stride, 0)[0], down[0].weight.grad, "downsample.0 dW")
 

@@ -6,7 +6,10 @@ masks, incoming gradients) and of the modules' parameters rounded to bf16 by tor
 packed weight layouts.  So no ReLU mask can flip between the engine and the reference, and each stage is held to the
 bound of a single launch: which packed weight slice a launch reads, the parity-class sub-grids of the stride-2 dgrads,
 which block's bit mask and bnp a fused reduction reads, where the downsample gradient lands and which arena slot receives
-each gradient are all checked at once.
+each gradient are all checked at once.  Bottleneck blocks (ResNet-50 / 101, Wide ResNet-50-2) and basic blocks
+(ResNet-18 / 34: conv1 3x3 strided, conv2 3x3, both weight gradients through the fp32 scratch and its unpack jobs; the
+identity blocks' conv1 dgrad adding the shortcut gradient under the block's bit mask and accumulating the previous
+block's bn2 sums under that block's mask) run through the same harness, dispatched on the tape's `basic` flag.
 
 Capture, without changing the engine: `eng._bn_fwd` / `eng._bn_act_fwd` / `eng._bn_bwd` are wrapped as instance
 attributes (statistics and running buffers before, bnp after; dA before, dy after, the arena's BN gradients before and
@@ -21,9 +24,10 @@ tests/gemm_reference.py for conv outputs, dgrads, the outgoing gradient and weig
 sums bounds of tests/test_backbone_kernels_gpu.py for dy, dgamma and dbeta.
 
 Power: each case prints one row per stage kind (run with -s): the worst err / bound and, for bf16 stages, the median of
-bound / |ref| (weight gradients: the largest bound over the RMS of the reference).  Each case asserts that the bounds
-are informative: median bound / |ref| <= BF16_INFO for every bf16 stage and max bound <= WGRAD_INFO * RMS for every
-weight gradient.  Set from a run on an H100 SXM (80 GB, default 700 W power limit), where every case took 21 s in all:
+bound / |ref| (weight gradients: the largest bound over the RMS of the reference), under a title that names the deepest
+weight-gradient launch.  Each case asserts that the bounds are informative: median bound / |ref| <= BF16_INFO for every
+bf16 stage and max bound <= its case's limit * RMS for every weight gradient.  Set from runs on an H100 SXM (80 GB,
+default 700 W power limit); the bottleneck cases:
   * bf16 stages: median bound / |ref| at most 0.0139 (the strided downsample of resnet101 at B = 1; about 1 bf16 ulp
     plus the accumulation term), BF16_INFO = 2^-6.  The worst err / bound of any bf16 stage was 0.5: half an ulp, the
     final rounding;
@@ -32,6 +36,20 @@ weight gradient.  Set from a run on an H100 SXM (80 GB, default 700 W power limi
     sum |terms|, about sqrt(rows) times |ref|: max bound / RMS 0.57 (stem), worst err / bound 0.027.  That case is held
     to WGRAD_INFO_B256 = 1, enough to catch a missing image tile, a wrong arena slot or a wrong operand; the small
     cases carry the tight check of the same launches.
+The basic-block cases (ResNet-18 / 34) and the bottleneck at a 288 crop, each case 1-2.5 s on the same machine (the
+figures move in the third digit between runs):
+  * bf16 stages: median bound / |ref| at most 0.0112 (the identity blocks' dx: the shortcut term added to the
+    bf16-rounded conv1 dgrad tile, two ulps) and 0.0127 for resnet50 at 288 (its stride-1 transition dx); worst
+    err / bound 0.5 in every case;
+  * weight gradients, max bound / RMS: 0.0023 (r18-b2-224), 0.0026 (r34-b2-224-fused-bn2-dynamic), 0.0050
+    (r18-b2-320), 0.0044 (r50-b2-288), all under WGRAD_INFO; 0.67 at B = 256 (r34-b256-224-dynamic, basic conv1),
+    worst err / bound 0.027, under WGRAD_INFO_B256;
+  * r18-b3-199x230-fused: 0.0118 (layer2.0's strided conv1; its downsample 0.0093).  Not looser data: the launch is
+    deeper.  Its wgrad reads the 25 x 29 output grid in boxes of 64 positions, and no power-of-two w x h box tiles a
+    29-wide grid without waste, so the kernel takes 1 x 1 x 64 boxes (one position of up to 64 images; three here):
+    725 k-blocks in 8 splits, L = 4 * 91 + 8 = 372 against 42 for the same conv at 224 x 224 at B = 2.  The bound
+    scales with L + 2; that case is held to WGRAD_INFO_DEEP = 2^-6, and its bound stays 85 times below the RMS.
+    resnet50 at the same extents stays under WGRAD_INFO (0.0070, its downsample) and keeps that limit.
 """
 import pytest
 import torch
@@ -39,6 +57,7 @@ import torch
 from oracle import virtex_oracle as O
 from tests import backbone_replica as R
 from tests import backbone_stages as S
+from tests import basic_oracle as BO
 from tests import gemm_reference as G
 from tests import wide_oracle as WO
 
@@ -47,6 +66,7 @@ pytestmark = pytest.mark.gpu
 BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
 BF16_INFO = 2.0 ** -6
 WGRAD_INFO = 2.0 ** -7
+WGRAD_INFO_DEEP = 2.0 ** -6
 WGRAD_INFO_B256 = 1.0
 
 
@@ -244,13 +264,22 @@ class Replay:
             self.check(kind, self.rows4(got, H, W), out.view(yv.shape))
             return pre
 
-        conv("fwd y1 conv1", x, name + ".conv1.weight", 1, 0, rec["y1"], Hi, Wi)
-        bnp1 = self.check_bnp(name + ".bn1", rec["bnp1"], rec["Min"])
-        act("fwd a1", rec["y1"], bnp1, rec["a1"], Hi, Wi)
-        conv(f"fwd y2 conv2 s{s}", self.rows4(rec["a1"], Hi, Wi), name + ".conv2.weight", s, 1, rec["y2"], Ho, Wo)
-        bnp2 = self.check_bnp(name + ".bn2", rec["bnp2"], rec["Mout"])
-        act("fwd a2", rec["y2"], bnp2, rec["a2"], Ho, Wo)
-        conv("fwd y3 conv3", self.rows4(rec["a2"], Ho, Wo), name + ".conv3.weight", 1, 0, rec["y3"], Ho, Wo)
+        if rec["basic"]:
+            # conv1 3x3 (stride) -> bn1 + ReLU -> conv2 3x3 -> bn2 + shortcut + ReLU, all at the output extent
+            conv(f"fwd y1 basic conv1 s{s}", x, name + ".conv1.weight", s, 1, rec["y1"], Ho, Wo)
+            bnp1 = self.check_bnp(name + ".bn1", rec["bnp1"], rec["Mout"])
+            act("fwd a1 basic", rec["y1"], bnp1, rec["a1"], Ho, Wo)
+            conv("fwd y2 basic conv2", self.rows4(rec["a1"], Ho, Wo), name + ".conv2.weight", 1, 1, rec["y2"], Ho, Wo)
+            last = "2"
+        else:
+            conv("fwd y1 conv1", x, name + ".conv1.weight", 1, 0, rec["y1"], Hi, Wi)
+            bnp1 = self.check_bnp(name + ".bn1", rec["bnp1"], rec["Min"])
+            act("fwd a1", rec["y1"], bnp1, rec["a1"], Hi, Wi)
+            conv(f"fwd y2 conv2 s{s}", self.rows4(rec["a1"], Hi, Wi), name + ".conv2.weight", s, 1, rec["y2"], Ho, Wo)
+            bnp2 = self.check_bnp(name + ".bn2", rec["bnp2"], rec["Mout"])
+            act("fwd a2", rec["y2"], bnp2, rec["a2"], Ho, Wo)
+            conv("fwd y3 conv3", self.rows4(rec["a2"], Ho, Wo), name + ".conv3.weight", 1, 0, rec["y3"], Ho, Wo)
+            last = "3"
         if rec["has_ds"]:
             assert s == 1 or rec["xs"] is None  # a stride-2 shortcut reads x in place (no subsampled copy)
             conv(f"fwd yd downsample s{s}", x, name + ".downsample.0.weight", s, 0, rec["yd"], Ho, Wo)
@@ -258,13 +287,13 @@ class Replay:
             res = self.rows4(rec["yd"], Ho, Wo)
         else:
             bnpd, res = None, x
-        bnp3 = self.check_bnp(name + ".bn3", rec["bnp3"], rec["Mout"])
-        pre = act("fwd block output", rec["y3"], bnp3, rec["out"], Ho, Wo, res=res.reshape(-1, res.shape[-1]),
-                  bnp_res=bnpd)
-        m3 = rec["m3"].view(self.B, Ho, Wo, -1)
-        m3 = m3 if self.sub is None else m3[self.sub]
-        assert torch.equal(m3.reshape(-1, m3.shape[-1]), R.pack_mask(pre > 0)), f"{name}: ReLU bit mask m3"
-        self.rows.setdefault("fwd bit mask m3", _Row("exact")).n += 1
+        bnpo = self.check_bnp(name + ".bn" + last, rec["bnp" + last], rec["Mout"])
+        pre = act("fwd block output" + (" basic" if rec["basic"] else ""), rec["y" + last], bnpo, rec["out"], Ho, Wo,
+                  res=res.reshape(-1, res.shape[-1]), bnp_res=bnpd)
+        m = rec["m" + last].view(self.B, Ho, Wo, -1)
+        m = m if self.sub is None else m[self.sub]
+        assert torch.equal(m.reshape(-1, m.shape[-1]), R.pack_mask(pre > 0)), f"{name}: ReLU bit mask m{last}"
+        self.rows.setdefault(f"fwd bit mask m{last}", _Row("exact")).n += 1
 
     # ------------------------------------------------------------------------------------------------ backward
     def bn_stage(self, kind, bn, dA, keep, y, bnp, dy_got, M, H, W, depth):
@@ -294,15 +323,27 @@ class Replay:
     def check_pending(self, dx):
         name, ref, bound = self.pending
         rec = self.recs[name]
-        self.check("bwd dx " + ("identity" if not rec["has_ds"] else f"transition s{rec['stride']}"),
+        self.check("bwd dx " + ("basic " if rec["basic"] else "") +
+                   ("identity" if not rec["has_ds"] else f"transition s{rec['stride']}"),
                    self.rows4(dx, rec["Hin"], rec["Win"]), ref, bound)
         self.pending = None
+
+    def downsample_bwd(self, rec, dA, keep, dy_got, depth):
+        """The downsample BN's share of a two-branch block-output BN backward, and its conv's weight gradient."""
+        name, Ho, Wo = rec["name"], rec["Hout"], rec["Wout"]
+        self.bn_stage("bwd dyd", name + ".downsample.1", dA, keep, rec["yd"], _d(rec["bnpd"]), dy_got, rec["Mout"],
+                      Ho, Wo, depth)
+        self.wgrad(name + ".downsample.0.weight", self.rows4(dy_got, Ho, Wo, full=True),
+                   self.rows4(rec["x"], rec["Hin"], rec["Win"], full=True), 1, rec["stride"], 0)
+        return self.rows4(dy_got, Ho, Wo)
 
     def on_bn_bwd(self, bn_name, dA, dys, two, depth):
         if bn_name == "visual.cnn.bn1":
             return self.on_stem_bwd(dA, dys[0], depth)
         name, which = bn_name.rsplit(".", 1)
         rec = self.recs[name]
+        if rec["basic"]:
+            return self.on_basic_bn_bwd(rec, which, dA, dys, two, depth)
         Hi, Wi, Ho, Wo, s = rec["Hin"], rec["Win"], rec["Hout"], rec["Wout"], rec["stride"]
         st = self.state = getattr(self, "state", None) if which != "bn3" else {}
         if which == "bn3":
@@ -315,10 +356,7 @@ class Replay:
             self.wgrad(name + ".conv3.weight", full(dys[0], Ho, Wo), full(rec["a2"], Ho, Wo), 1, 1, 0)
             st["dy3"] = self.rows4(dys[0], Ho, Wo)
             if two:
-                self.bn_stage("bwd dyd", name + ".downsample.1", dA, keep, rec["yd"], _d(rec["bnpd"]), dys[1],
-                              rec["Mout"], Ho, Wo, depth)
-                self.wgrad(name + ".downsample.0.weight", full(dys[1], Ho, Wo), full(rec["x"], Hi, Wi), 1, s, 0)
-                st["dyd"] = self.rows4(dys[1], Ho, Wo)
+                st["dyd"] = self.downsample_bwd(rec, dA, keep, dys[1], depth)
             else:
                 st["dOut"] = self.rows4(dA, Ho, Wo)
                 k = keep.view(self.B, Ho, Wo, -1)
@@ -353,6 +391,45 @@ class Replay:
             self.pending = (name, ref, bound)
             self.state = None
 
+    def on_basic_bn_bwd(self, rec, which, dA, dys, two, depth):
+        """A basic block's backward: bn2 (+ the downsample BN) from the block's output gradient, conv2's 3x3 dgrad
+        da1 read by bn1, and conv1's strided 3x3 dgrad (+ shortcut) left pending for the stage that reads it."""
+        name, Hi, Wi, Ho, Wo, s, C = (rec["name"], rec["Hin"], rec["Win"], rec["Hout"], rec["Wout"], rec["stride"],
+                                      rec["Cout"])
+        bn_name = name + "." + which
+        if which == "bn2":
+            if self.pending is not None:
+                self.check_pending(dA)
+            st = self.state = {}
+            keep = R.unpack_mask(rec["m2"], C)
+            self.bn_stage("bwd dy2 basic", bn_name, dA, keep, rec["y2"], _d(rec["bnp2"]), dys[0], rec["Mout"], Ho, Wo,
+                          depth)
+            self.wgrad(name + ".conv2.weight", self.rows4(dys[0], Ho, Wo, full=True),
+                       self.rows4(rec["a1"], Ho, Wo, full=True), 3, 1, 1)
+            st["dy2"] = self.rows4(dys[0], Ho, Wo)
+            if two:
+                st["dyd"] = self.downsample_bwd(rec, dA, keep, dys[1], depth)
+            else:
+                st["dOut"] = self.rows4(dA, Ho, Wo)
+                k = keep.view(self.B, Ho, Wo, -1)
+                st["keep2"] = k if self.sub is None else k[self.sub]
+            return
+        st = self.state
+        ref, mag = S.conv_dgrad(st["dy2"], self.w(name + ".conv2.weight"), 1, 1, Ho, Wo)
+        self.check("bwd da1 basic conv2 dgrad", self.rows4(dA, Ho, Wo), ref, S.bf16_bound(ref, S.gemm_err(mag, 9 * C)))
+        bnp1 = _d(rec["bnp1"])
+        keep = S.relu_keep(_d(rec["y1"]), bnp1)
+        self.bn_stage("bwd dy1 basic", bn_name, dA, keep, rec["y1"], bnp1, dys[0], rec["Mout"], Ho, Wo, depth)
+        self.wgrad(name + ".conv1.weight", self.rows4(dys[0], Ho, Wo, full=True),
+                   self.rows4(rec["x"], Hi, Wi, full=True), 3, s, 1)
+        dy1, w1 = self.rows4(dys[0], Ho, Wo), self.w(name + ".conv1.weight")
+        if rec["has_ds"]:
+            ref, bound = S.basic_block_dx(dy1, w1, s, Hi, Wi, dyd=st["dyd"], wd=self.w(name + ".downsample.0.weight"))
+        else:
+            ref, bound = S.basic_block_dx(dy1, w1, s, Hi, Wi, dOut=st["dOut"], keep2=st["keep2"])
+        self.pending = (name, ref, bound)
+        self.state = None
+
     def on_maxpool_bwd(self, ptr):
         ws = self.eng.ws.flat
         names = [n for n in ("bwd.dx0", "bwd.dx1") if n in ws and ws[n].data_ptr() == ptr]
@@ -378,14 +455,17 @@ class Replay:
     def check_weight_grads(self):
         e = self.eng
         for wname, (ref, mag) in sorted(self.wref.items()):
-            if wname == "visual.cnn.conv1.weight":
-                ptr = e._dwp["visual.cnn.conv1"].data_ptr()
-            elif wname.endswith(".conv2.weight"):
-                ptr = e._dwp[wname[:-len(".weight")]].data_ptr()
+            # every k > 1 conv (the stem, conv2 of a bottleneck, both 3x3 convs of a basic block) accumulates into
+            # its fp32 scratch, which the unpack jobs fold into the arena; the 1x1 convs straight into the arena
+            key = wname[:-len(".weight")]
+            ptr = (e._dwp[key] if key in e._dwp else e.G(wname)).data_ptr()
+            if "layer" not in wname:
+                kind = "bwd dW stem"
+            elif "downsample" in wname:
+                kind = "bwd dW downsample"
             else:
-                ptr = e.G(wname).data_ptr()
-            kind = "bwd dW " + ("stem" if "layer" not in wname else
-                                "downsample" if "downsample" in wname else wname.split(".")[-2])
+                kind = "bwd dW " + ("basic " if self.recs[wname.rsplit(".", 2)[0]]["basic"] else "") + \
+                    wname.split(".")[-2]
             self.check(kind, e.G(wname), ref, S.wgrad_bound(mag, self.wdepth[ptr]), info="wgrad")
         assert len(self.wref) == sum(1 for n in e.arena.names if n.startswith("visual.") and n.endswith("weight")
                                      and len(e.arena.shapes[n]) == 4)
@@ -410,6 +490,21 @@ class Replay:
 
         def bnp(bn):
             return _d(ws["bnp_eval:" + bn].view(4, -1))
+        if rec["basic"]:
+            # conv1 3x3 (stride) with bn1 folded + ReLU, then conv2 3x3 with bn2 folded + shortcut + ReLU
+            if n == "inf.a1":
+                ref, bound = S.eval_conv_bn(x, self.w(name + ".conv1.weight"), s, 1, bnp(name + ".bn1"))
+                self.check(f"eval a1 basic s{s}", self.rows4(D, Ho, Wo), ref, bound)
+                es["a1"] = D
+                return
+            if n != "inf.shortcut":
+                assert kw.get("residual") is not None, n
+                want = es.pop("shortcut", None)
+                assert kw["residual"].data_ptr() == (es["x"] if want is None else want).data_ptr(), f"{name}: shortcut"
+                ref, bound = S.eval_conv_bn(self.rows4(es["a1"], Ho, Wo), self.w(name + ".conv2.weight"), 1, 1,
+                                            bnp(name + ".bn2"), res=self.rows4(kw["residual"], Ho, Wo))
+                self.check("eval block output basic", self.rows4(D, Ho, Wo), ref, bound)
+                return
         if n == "inf.a1":
             ref, bound = S.eval_conv_bn(x, self.w(name + ".conv1.weight"), 1, 0, bnp(name + ".bn1"))
             self.check("eval a1", self.rows4(D, Hi, Wi), ref, bound)
@@ -462,8 +557,12 @@ def eng_sms():
 def _model(backbone, seed):
     from virtex_b200.models import VirTexModel
     from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    spec = WO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
-    state = WO.synth_state(spec, seed, bn3_gain=0.25)
+    if backbone in BO.BLOCKS:
+        spec = BO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
+        state = BO.synth_state(spec, seed, residual_gain=0.25)
+    else:
+        spec = WO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
+        state = WO.synth_state(spec, seed, bn3_gain=0.25)
     visual = TorchvisionVisualBackbone(backbone, visual_feature_size=spec.visual_feature_size)
     textual = TransformerDecoderTextualHead(
         visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
@@ -474,18 +573,25 @@ def _model(backbone, seed):
     return model.cuda().train()
 
 
-CASES = [  # id, backbone, B, (H, W), fuse_bn3_min_rows (None: default), dynamic schedule, eval replay
-    pytest.param("resnet50", 2, (224, 224), None, False, True, id="r50-b2-224"),
-    pytest.param("resnet50", 2, (224, 224), 0, True, False, id="r50-b2-224-fused-bn3-dynamic"),
-    pytest.param("resnet50", 3, (199, 230), None, False, True, id="r50-b3-199x230"),
-    pytest.param("wide_resnet50_2", 2, (224, 224), None, False, True, id="r50w2x-b2-224"),
-    pytest.param("resnet101", 1, (224, 224), None, False, False, id="r101-b1-224"),
-    pytest.param("resnet50", 256, (224, 224), None, True, False, id="r50-b256-224-dynamic"),
+CASES = [  # backbone, B, (H, W), fuse_bn3_min_rows (None: default), dynamic schedule, eval replay, weight-gradient
+    # informativeness limit (max bound / RMS)
+    pytest.param("resnet50", 2, (224, 224), None, False, True, WGRAD_INFO, id="r50-b2-224"),
+    pytest.param("resnet50", 2, (224, 224), 0, True, False, WGRAD_INFO, id="r50-b2-224-fused-bn3-dynamic"),
+    pytest.param("resnet50", 3, (199, 230), None, False, True, WGRAD_INFO, id="r50-b3-199x230"),
+    pytest.param("wide_resnet50_2", 2, (224, 224), None, False, True, WGRAD_INFO, id="r50w2x-b2-224"),
+    pytest.param("resnet101", 1, (224, 224), None, False, False, WGRAD_INFO, id="r101-b1-224"),
+    pytest.param("resnet50", 256, (224, 224), None, True, False, WGRAD_INFO_B256, id="r50-b256-224-dynamic"),
+    pytest.param("resnet18", 2, (224, 224), None, False, True, WGRAD_INFO, id="r18-b2-224"),
+    pytest.param("resnet34", 2, (224, 224), 0, True, False, WGRAD_INFO, id="r34-b2-224-fused-bn2-dynamic"),
+    pytest.param("resnet18", 3, (199, 230), 0, False, True, WGRAD_INFO_DEEP, id="r18-b3-199x230-fused"),
+    pytest.param("resnet34", 256, (224, 224), None, True, False, WGRAD_INFO_B256, id="r34-b256-224-dynamic"),
+    pytest.param("resnet18", 2, (320, 320), None, False, True, WGRAD_INFO, id="r18-b2-320"),
+    pytest.param("resnet50", 2, (288, 288), None, False, True, WGRAD_INFO, id="r50-b2-288"),
 ]
 
 
-@pytest.mark.parametrize("backbone,B,hw,fuse_rows,dynamic,with_eval", CASES)
-def test_backbone_stages_replay(backbone, B, hw, fuse_rows, dynamic, with_eval, monkeypatch):
+@pytest.mark.parametrize("backbone,B,hw,fuse_rows,dynamic,with_eval,wgrad_info", CASES)
+def test_backbone_stages_replay(backbone, B, hw, fuse_rows, dynamic, with_eval, wgrad_info, monkeypatch):
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
     from virtex_b200 import ops
@@ -512,5 +618,5 @@ def test_backbone_stages_replay(backbone, B, hw, fuse_rows, dynamic, with_eval, 
         torch.cuda.synchronize()
     finally:
         ops.set_dynamic_gemm_schedule(False)
-    rp.report(f"{backbone} B={B} {hw[0]}x{hw[1]} fuse_bn3_min_rows={eng.fuse_bn3_min_rows} dynamic={int(dynamic)}",
-              WGRAD_INFO if B < 256 else WGRAD_INFO_B256)
+    rp.report(f"{backbone} B={B} {hw[0]}x{hw[1]} fuse_bn3_min_rows={eng.fuse_bn3_min_rows} dynamic={int(dynamic)} "
+              f"deepest weight-gradient launch L={max(rp.wdepth.values())}", wgrad_info)

@@ -13,7 +13,12 @@ fusion in every identity block.
 
 Then the backbone and the model against the float64 oracle of tests/basic_oracle.py with the bounds of
 tests/test_wide_resnet_gpu.py, the model against the reference's fixture, the downstream forward against torchvision's
-resnet18 / resnet34 in float64, six Trainer steps, a beam search, and batch-256 steps of R18-L1-H1024 and R34-L1-H1024."""
+resnet18 / resnet34 in float64, six Trainer steps, a beam search, and batch-256 steps of R18-L1-H1024 and R34-L1-H1024.
+
+The GEMM check proves that each launch computes what its arguments say, and the oracle comparisons are loose (relative
+L2, cosine); neither proves that the engine passed the right mask, y, bnp, sub-grid or arena slot.  That wiring is
+checked element by element in tests/test_backbone_stages_gpu.py, which replays every stage of both nets (forward,
+backward, weight gradients and the eval forward) against float64 references of the engine's own stage inputs."""
 import os
 
 import pytest
