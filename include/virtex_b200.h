@@ -431,7 +431,12 @@ int vtx_jpeg_color(const int32_t* info, const int64_t* info64, const uint8_t* pl
  * virtex/optim/lookahead.py:82-102).  segs: device array of {int64 begin, int64 end, float lr, float wd}.
  * ctl[0] = gradient scale (clip / world size), ctl[1] = gradient norm; hyper = {lr multiplier, first step, lookahead}.
  * ------------------------------------------------------------------------------------------------------------------ */
+/* *out += sum of x[i]^2 over n elements (n = 0 leaves *out untouched); x must be 16-byte aligned (read as float4). */
 int vtx_sumsq(const float* x, int64_t n, float* out, void* stream);
+/* norm = sqrt(*sumsq) / world_size; ctl = {min(1, max_norm / (norm + 1e-6)) / world_size, norm}.  Non-finite norms
+ * follow torch.nn.utils.clip_grad_norm_: an inf norm gives the coefficient 0 and a NaN norm a NaN coefficient, so the
+ * step writes NaN into every updated parameter (the step is not skipped, as a GradScaler would).  max_norm <= 0
+ * disables clipping (coefficient 1 / world_size), where clip_grad_norm_ would scale every gradient by <= 0. */
 int vtx_clip_coef(const float* sumsq, int world_size, float max_norm, float* ctl, void* stream);
 int vtx_sgd_step(float* p, const float* g, float* mom, float* slow, void* p_bf, const void* segs, int nseg,
                  const float* ctl, const float* hyper, float momentum, float la_alpha, void* stream);

@@ -527,7 +527,9 @@ def test_dropout_runs_and_is_unbiased():
 
 # ------------------------------------------------------------------------------------------------- optimiser / trainer
 def test_sgd_step_kernel_matches_reference_arithmetic():
-    """vtx_sgd_step == torch.optim.SGD(momentum, per-tensor lr/wd) + Lookahead arithmetic on random arenas."""
+    """vtx_sgd_step == torch.optim.SGD(momentum, per-tensor lr/wd) + Lookahead arithmetic on random arenas, in fp32.
+    The element-level float64 checks of the whole tail (vtx_sumsq, vtx_clip_coef, vtx_sgd_step with gaps and frozen
+    tensors, Trainer steps replayed from their own gradients, the bucket contract) are in tests/test_sgd_tail_gpu.py."""
     _need_cuda()
     import struct
     from virtex_b200.ops import call, _stream

@@ -31,11 +31,13 @@ __global__ void sumsq_kernel(const float* __restrict__ x, long long n, float* __
 }
 
 // ctl[0] = grad scale applied in the update = (1/world) * min(1, max_norm / (norm + 1e-6)),  ctl[1] = norm of the mean grad
+// The clamp keeps a NaN coefficient, as torch.clamp(coef, max=1) in clip_grad_norm_ does (fminf would return 1 and
+// let a NaN-norm step run unclipped); an inf norm gives 0.  max_norm <= 0 means no clipping.
 __global__ void clip_coef_kernel(const float* __restrict__ sumsq, float inv_world, float max_norm, float* __restrict__ ctl) {
   VTX_PDL_TRIGGER();
   const float norm = sqrtf(*sumsq) * inv_world;
   float c = max_norm > 0.f ? max_norm / (norm + 1e-6f) : 1.f;
-  c = fminf(c, 1.f);
+  c = c > 1.f ? 1.f : c;
   ctl[0] = c * inv_world;
   ctl[1] = norm;
 }

@@ -9,6 +9,10 @@ torch.optim.SGD or torch.optim.AdamW (OPTIM.OPTIMIZER_NAME "sgd" / "adamw"; Adam
 as the reference) + virtex/optim/lookahead.py + virtex/optim/lr_scheduler.py; bf16 needs no GradScaler.  SGD keeps a
 momentum arena; AdamW keeps exp_avg / exp_avg_sq arenas and one host-side step count t, from which the host computes
 the bias corrections in double precision for each step.
+Non-finite gradients follow torch.nn.utils.clip_grad_norm_: a NaN norm makes the clip coefficient NaN and the step
+writes NaN into every trainable parameter; an inf norm gives the coefficient 0.  GradScaler's skip-on-non-finite is not
+reproduced: skipping on the device would need the Lookahead counter and the first-step momentum flag, which the host
+keeps, to move to the device as well.  CLIP_GRAD_NORM <= 0 disables clipping.
 Gradient all-reduce: NCCL over NVLink on a side stream, one bucket per completed gradient range in backward order
 (backward-direction decoder; forward-direction decoder + shared embedding / projection; layer4; layer3; layer2; the
 rest), SUM on the wire and the 1/world_size folded into the clip coefficient,
