@@ -12,7 +12,10 @@ a reference checkout (`oracle/make_golden.py`), and the resulting fixtures are c
 
 Reference call sites restated (file:line, relative to the reference root unless prefixed SP/ = site-packages):
   * ResNet-v1.5 to layer4          virtex/modules/visual_backbones.py:43-74 -> SP/torchvision/models/resnet.py:108-163,
-                                   166-285 (Bottleneck, stride on the 3x3, zero_init_residual)
+                                   166-285 (Bottleneck, stride on the 3x3, zero_init_residual; wide: width_per_group
+                                   128, :922-985)
+  * basic-block ResNet-18 / 34     SP/torchvision/models/resnet.py:59-105 (BasicBlock: conv1 3x3 carries the stride,
+                                   conv2 3x3, expansion 1, 512 output channels)
   * BatchNorm2d (train / eval)     SP/torchvision/models/resnet.py:147-155 (SURVEY Appendix C.2)
   * visual projection + embedding  virtex/modules/textual_heads.py:240-259, virtex/modules/embedding.py:46-74
   * post-/pre-norm decoder layer   SP/torch/nn/modules/transformer.py:1131-1199; MHA SP/torch/nn/functional.py:6244-6690
@@ -26,13 +29,24 @@ from __future__ import annotations
 import math
 import re
 from collections import OrderedDict
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
 
-_RESNET_LAYERS = {"resnet50": [3, 4, 6, 3], "resnet101": [3, 4, 23, 3], "resnet152": [3, 8, 36, 3]}
+_RESNET_LAYERS = {"resnet18": [2, 2, 2, 2], "resnet34": [3, 4, 6, 3], "resnet50": [3, 4, 6, 3],
+                  "resnet101": [3, 4, 23, 3], "resnet152": [3, 8, 36, 3], "wide_resnet50_2": [3, 4, 6, 3],
+                  "wide_resnet101_2": [3, 4, 23, 3]}
+# (block kind, width per group), as torchvision's constructors set them: a basic block is two 3x3 convs of `planes`
+# channels; a bottleneck is planes * width_per_group / 64 channels wide inside and 4 * planes at its output.
+_RESNET_BLOCK = {"resnet18": ("basic", 64), "resnet34": ("basic", 64), "resnet50": ("bottleneck", 64),
+                 "resnet101": ("bottleneck", 64), "resnet152": ("bottleneck", 64),
+                 "wide_resnet50_2": ("bottleneck", 128), "wide_resnet101_2": ("bottleneck", 128)}
+
+
+def _is_basic(spec: "Spec") -> bool:
+    return _RESNET_BLOCK[spec.backbone][0] == "basic"
 
 
 @dataclass
@@ -47,7 +61,7 @@ class Spec:
     vocab: int = 10000
     max_len: int = 30
     pad: int = 0
-    visual_feature_size: int = 2048
+    visual_feature_size: Optional[int] = None  # default: the backbone's output width, 512 (basic blocks) or 2048
     caption_backward: bool = True
     mask_future: bool = True  # False: masked language modelling (virtex/factories.py:395 -> textual_heads.py:255-262)
     blocks: List[int] = field(default_factory=list)
@@ -55,11 +69,16 @@ class Spec:
     def __post_init__(self):
         if not self.blocks:
             self.blocks = list(_RESNET_LAYERS[self.backbone])
+        if self.visual_feature_size is None:
+            self.visual_feature_size = 512 if _is_basic(self) else 2048
 
 
 # ----------------------------------------------------------------------------------------------- parameter inventory
 def backbone_param_shapes(spec: Spec) -> "OrderedDict[str, Tuple[int, ...]]":
     """Names/shapes of `visual.cnn.*` parameters and buffers, in torchvision registration order."""
+    kind, width_per_group = _RESNET_BLOCK[spec.backbone]
+    basic = kind == "basic"
+    k1, expansion = (3, 1) if basic else (1, 4)  # basic: conv1 3x3, conv2 3x3; bottleneck: 1x1, 3x3, 1x1 (conv3)
     out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
 
     def bn(prefix, c):
@@ -74,19 +93,21 @@ def backbone_param_shapes(spec: Spec) -> "OrderedDict[str, Tuple[int, ...]]":
     bn(p + "bn1", 64)
     inplanes = 64
     for li, (planes, nblocks) in enumerate(zip([64, 128, 256, 512], spec.blocks), start=1):
+        width = planes * width_per_group // 64
         for bi in range(nblocks):
             stride = 2 if (bi == 0 and li > 1) else 1
             q = f"{p}layer{li}.{bi}."
-            out[q + "conv1.weight"] = (planes, inplanes, 1, 1)
-            bn(q + "bn1", planes)
-            out[q + "conv2.weight"] = (planes, planes, 3, 3)
-            bn(q + "bn2", planes)
-            out[q + "conv3.weight"] = (planes * 4, planes, 1, 1)
-            bn(q + "bn3", planes * 4)
-            if stride != 1 or inplanes != planes * 4:
-                out[q + "downsample.0.weight"] = (planes * 4, inplanes, 1, 1)
-                bn(q + "downsample.1", planes * 4)
-            inplanes = planes * 4
+            out[q + "conv1.weight"] = (width, inplanes, k1, k1)
+            bn(q + "bn1", width)
+            out[q + "conv2.weight"] = (width, width, 3, 3)
+            bn(q + "bn2", width)
+            if not basic:
+                out[q + "conv3.weight"] = (planes * expansion, width, 1, 1)
+                bn(q + "bn3", planes * expansion)
+            if stride != 1 or inplanes != planes * expansion:
+                out[q + "downsample.0.weight"] = (planes * expansion, inplanes, 1, 1)
+                bn(q + "downsample.1", planes * expansion)
+            inplanes = planes * expansion
     return out
 
 
@@ -166,12 +187,25 @@ def synth_state(spec: Spec, seed: int = 0, randomize_bn: bool = True,
     Scales follow the reference initialisers (Kaiming fan_out convs, N(0, 0.02) head weights) but BN affine
     parameters and running statistics are randomised when `randomize_bn` so that every gradient is exercised
     (fresh `zero_init_residual` makes 112 of 202 gradients identically zero; SURVEY section 8c gotcha (i)).
-    `bn3_gain` scales the last BN gamma of every bottleneck: with gain 1 a random 16-block residual stack amplifies any
+    `bn3_gain` scales the last BN gamma of every residual block (bn3 of a bottleneck, bn2 of a basic block; zero
+    without `randomize_bn`, as zero_init_residual): with gain 1 a random 16-block residual stack amplifies any
     perturbation ~1.25x per block (bf16 rounding -> 50% feature error at layer4), which is a property of that random
-    network, not of an implementation; bf16-vs-fp32 parity tests therefore use a residual branch gain of ~0.25."""
-    g = torch.Generator().manual_seed(seed)
+    network, not of an implementation; bf16-vs-fp32 parity tests therefore use a residual branch gain of ~0.25.
+
+    ResNet-50/101/152 draw every tensor in `unique_shapes` order from one generator seeded `seed`.  The wide and
+    basic-block backbones draw theirs in registration order from a generator of their own, seeded 10_000 + seed and
+    20_000 + seed, and take the textual tensors that the same head draws on a resnet50 backbone."""
+    kind, width_per_group = _RESNET_BLOCK[spec.backbone]
+    own_generator = kind == "basic" or width_per_group != 64
+    if own_generator:
+        g = torch.Generator().manual_seed((20_000 if kind == "basic" else 10_000) + seed)
+        shapes = backbone_param_shapes(spec)
+    else:
+        g = torch.Generator().manual_seed(seed)
+        shapes = unique_shapes(spec)
+    last_bn = ".bn2." if kind == "basic" else ".bn3."
     out: "OrderedDict[str, torch.Tensor]" = OrderedDict()
-    for name, shape in unique_shapes(spec).items():
+    for name, shape in shapes.items():
         if name.endswith("num_batches_tracked"):
             t = torch.zeros((), dtype=torch.int64)
         elif name.endswith("running_mean"):
@@ -183,9 +217,9 @@ def synth_state(spec: Spec, seed: int = 0, randomize_bn: bool = True,
             t = torch.randn(shape, generator=g) * math.sqrt(2.0 / fan_out)
         elif "visual.cnn" in name and name.endswith(".weight"):  # BN gamma
             t = torch.rand(shape, generator=g) + 0.5 if randomize_bn else torch.ones(shape)
-            if not randomize_bn and ".bn3." in name:
+            if not randomize_bn and last_bn in name:
                 t = torch.zeros(shape)
-            elif ".bn3." in name:
+            elif last_bn in name:
                 t = t * bn3_gain
         elif "visual.cnn" in name:  # BN beta
             t = torch.randn(shape, generator=g) * 0.1 if randomize_bn else torch.zeros(shape)
@@ -200,6 +234,10 @@ def synth_state(spec: Spec, seed: int = 0, randomize_bn: bool = True,
             if name == "textual.embedding.words.weight":
                 t[spec.pad].zero_()
         out[name] = t
+    if own_generator:
+        head = synth_state(replace(spec, backbone="resnet50", blocks=list(_RESNET_LAYERS["resnet50"])), seed,
+                           randomize_bn, bn3_gain)
+        out.update((k, v) for k, v in head.items() if not k.startswith("visual."))
     return out
 
 
@@ -268,8 +306,9 @@ def _batch_norm(x, P, prefix, training, new_buffers, eps=1e-5, momentum=0.1, emu
 
 
 def backbone_forward(P, image, spec: Spec, training=True, new_buffers=None, record=None, emulate_bf16=False):
-    """(B,3,H,W) -> (B,2048,H/32,W/32).  torchvision ResNet children conv1..layer4.
-    `record` (dict) optionally receives intermediate activations keyed by layer name (debug / per-layer parity)."""
+    """(B,3,H,W) -> (B,C,H/32,W/32), C = 512 for basic blocks and 2048 otherwise.  torchvision ResNet children
+    conv1..layer4.  `record` (dict) optionally receives the stem's and every block's intermediates (y1, a1, y2, out)."""
+    basic = _is_basic(spec)
     p = "visual.cnn."
     rb = _rb if emulate_bf16 else (lambda t: t)
     bn = lambda t, name: _batch_norm(t, P, name, training, new_buffers, emulate_bf16=emulate_bf16)
@@ -285,18 +324,22 @@ def backbone_forward(P, image, spec: Spec, training=True, new_buffers=None, reco
             stride = 2 if (bi == 0 and li > 1) else 1
             q = f"{p}layer{li}.{bi}."
             identity = x
-            out = F.conv2d(x, rb(P[q + "conv1.weight"]))
+            # the first 3x3 conv carries the stride: conv1 of a basic block, conv2 of a bottleneck
+            out = F.conv2d(x, rb(P[q + "conv1.weight"]), stride=stride if basic else 1, padding=1 if basic else 0)
             if record is not None:
                 record[q + "y1"] = out
             out = rb(torch.relu(bn(out, q + "bn1")))
             if record is not None:
                 record[q + "a1"] = out
-            out = F.conv2d(out, rb(P[q + "conv2.weight"]), stride=stride, padding=1)
+            out = F.conv2d(out, rb(P[q + "conv2.weight"]), stride=1 if basic else stride, padding=1)
             if record is not None:
                 record[q + "y2"] = out
-            out = rb(torch.relu(bn(out, q + "bn2")))
-            out = F.conv2d(out, rb(P[q + "conv3.weight"]))
-            out = bn(out, q + "bn3")
+            if basic:
+                out = bn(out, q + "bn2")
+            else:
+                out = rb(torch.relu(bn(out, q + "bn2")))
+                out = F.conv2d(out, rb(P[q + "conv3.weight"]))
+                out = bn(out, q + "bn3")
             if q + "downsample.0.weight" in P:
                 identity = F.conv2d(x, rb(P[q + "downsample.0.weight"]), stride=stride)
                 identity = bn(identity, q + "downsample.1")

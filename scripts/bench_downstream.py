@@ -92,7 +92,8 @@ def main():
         raise SystemExit("bench_downstream.py measures the GPU path: no CUDA device")
     import torchvision
     from virtex_b200.modules import ResNetParams
-    from tests import basic_oracle as BO, downstream_oracle as DO, wide_oracle as WO
+    from oracle import virtex_oracle as O
+    from tests import downstream_oracle as DO
 
     print(f"card: {card()}", flush=True)
     torch.manual_seed(0)
@@ -101,12 +102,8 @@ def main():
     if a.arch == "resnet50":
         state = DO.synth_state(0, a.classes)
     else:  # the same recipe on the other architecture's parameter tree
-        if a.arch in BO.BLOCKS:
-            spec = BO.spec(a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
-            full = BO.synth_state(spec, 0, residual_gain=0.25)
-        else:
-            spec = WO.spec(a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
-            full = WO.synth_state(spec, 0, bn3_gain=0.25)
+        spec = O.Spec(backbone=a.arch, hidden=128, layers=1, heads=2, ffn=256, caption_backward=False)
+        full = O.synth_state(spec, 0, bn3_gain=0.25)
         state = {k[len(DO.PREFIX):]: v for k, v in full.items() if k.startswith(DO.PREFIX)}
         g = torch.Generator().manual_seed(7000)
         state["fc.weight"] = torch.randn(a.classes, width, generator=g) * 0.01

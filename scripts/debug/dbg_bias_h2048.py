@@ -3,7 +3,8 @@ import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import torch
 from oracle import virtex_oracle as O
-from tests.test_gpu_parity import build_model, to_cuda, rel, cos
+from tests.helpers import build_model, to_cuda
+from tests.test_gpu_parity import rel, cos
 
 for kw in (dict(backbone="resnet101", hidden=2048, heads=32, ffn=8192), dict(hidden=2048, heads=32, ffn=8192),
            dict(backbone="resnet101")):

@@ -6,7 +6,7 @@ $VIRTEX_REFERENCE_ROOT) on the CPU:
 The basic-block sibling of scripts/make_wide_golden.py: the reference's VirTexModel with
 TorchvisionVisualBackbone("resnet18", visual_feature_size=512) (MODEL.VISUAL.NAME torchvision::resnet18 with
 MODEL.VISUAL.FEATURE_SIZE 512) and a small post-norm head, batch 2, in float64 and float32, with weights from
-tests/basic_oracle.py.  Only the reference's outputs are stored, in the layout of the other model fixtures: training
+oracle/virtex_oracle.py.  Only the reference's outputs are stored, in the layout of the other model fixtures: training
 loss and its components, gradient norms / sums / probes, BN buffers, and the eval-mode loss, predictions, logits and
 features."""
 import os
@@ -19,10 +19,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import ref_shim, virtex_oracle as O  # noqa: E402
 from oracle.make_golden import build_reference_model, grad_summary  # noqa: E402
-from tests import basic_oracle as BO  # noqa: E402
 
 NAME = "r18_l1_h128_post_b2"
-SPEC = dict(backbone="resnet18", hidden=128, layers=1, heads=2, ffn=256)  # basic_oracle.spec(**SPEC)
+SPEC = dict(backbone="resnet18", hidden=128, layers=1, heads=2, ffn=256)  # O.Spec(**SPEC)
 BATCH = dict(batch_size=2, seed=5, ragged=False)
 SEED = 5
 PROBES = ("visual.cnn.conv1.weight", "visual.cnn.layer1.0.conv1.weight", "visual.cnn.layer4.1.conv2.weight",
@@ -36,8 +35,8 @@ def main():
     warnings.filterwarnings("ignore")
     ref_shim.install()
     torch.manual_seed(0)
-    spec = BO.spec(**SPEC)
-    state = BO.synth_state(spec, SEED)
+    spec = O.Spec(**SPEC)
+    state = O.synth_state(spec, SEED)
     batch = O.synth_batch(max_len=spec.max_len, vocab=spec.vocab, **BATCH)
     out = {"spec": SPEC, "batch": BATCH, "seed": SEED}
     for tag, dtype in (("f64", torch.float64), ("f32", torch.float32)):

@@ -5,7 +5,7 @@ $VIRTEX_REFERENCE_ROOT) on the CPU:
 
 The wide sibling of oracle/make_golden.py's cases: the reference's VirTexModel with
 TorchvisionVisualBackbone("wide_resnet50_2") (the R_50W2X backbone ablation) and a small post-norm head, batch 2, in
-float64 and float32, with weights from tests/wide_oracle.py.  Only the reference's outputs are stored, in the layout
+float64 and float32, with weights from oracle/virtex_oracle.py.  Only the reference's outputs are stored, in the layout
 of the other model fixtures: training loss and its components, gradient norms / sums / probes, BN buffers, and the
 eval-mode loss, predictions, logits and features."""
 import os
@@ -18,10 +18,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import ref_shim, virtex_oracle as O  # noqa: E402
 from oracle.make_golden import build_reference_model, grad_summary  # noqa: E402
-from tests import wide_oracle as WO  # noqa: E402
 
 NAME = "r50w2x_l1_h128_post_b2"
-SPEC = dict(backbone="wide_resnet50_2", hidden=128, layers=1, heads=2, ffn=256)  # wide_oracle.spec(**SPEC)
+SPEC = dict(backbone="wide_resnet50_2", hidden=128, layers=1, heads=2, ffn=256)  # O.Spec(**SPEC)
 BATCH = dict(batch_size=2, seed=5, ragged=False)
 SEED = 5
 PROBES = ("visual.cnn.conv1.weight", "visual.cnn.layer4.2.conv3.weight", "textual.embedding.words.weight",
@@ -34,8 +33,8 @@ def main():
     warnings.filterwarnings("ignore")
     ref_shim.install()
     torch.manual_seed(0)
-    spec = WO.spec(**SPEC)
-    state = WO.synth_state(spec, SEED)
+    spec = O.Spec(**SPEC)
+    state = O.synth_state(spec, SEED)
     batch = O.synth_batch(max_len=spec.max_len, vocab=spec.vocab, **BATCH)
     out = {"spec": SPEC, "batch": BATCH, "seed": SEED}
     for tag, dtype in (("f64", torch.float64), ("f32", torch.float32)):

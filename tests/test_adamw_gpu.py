@@ -113,7 +113,7 @@ def test_adamw_trainer_trajectory_vs_oracle():
     """6 fused AdamW steps (crossing the Lookahead boundary) track the float64 AdamW oracle on losses and gradient
     norms, and every step's update equals float64 AdamW applied to the trainer's own clipped gradient arena."""
     _need_cuda()
-    from tests.test_gpu_parity import build_model, to_cuda
+    from tests.helpers import build_model, to_cuda
     from virtex_b200.trainer import Trainer
     spec = O.Spec(hidden=128, layers=1, heads=2, ffn=256)
     state = O.synth_state(spec, 3, bn3_gain=0.25)
@@ -151,7 +151,7 @@ def _resume_config():
 def test_adamw_trainer_checkpoint_resume_matches_uninterrupted_run(tmp_path):
     """3 steps -> CheckpointManager.step -> fresh model + Trainer -> load -> 3 more steps == 6 uninterrupted steps."""
     _need_cuda()
-    from tests.test_gpu_parity import to_cuda
+    from tests.helpers import to_cuda
     from virtex_b200.checkpointing import CheckpointManager
     from virtex_b200.factories import PretrainingModelFactory
     from virtex_b200.trainer import Trainer
@@ -184,7 +184,7 @@ def test_adamw_trainer_continues_a_checkpoint_of_the_eager_torch_loop(tmp_path):
     """The eager loop (autograd on the engine, clip_grad_norm_, torch.optim.AdamW on CUDA, LambdaLR) writes a checkpoint
     after 3 steps; a fresh Trainer loads it and its next 3 losses follow the eager loop's next 3."""
     _need_cuda()
-    from tests.test_gpu_parity import to_cuda
+    from tests.helpers import to_cuda
     from virtex_b200.checkpointing import CheckpointManager
     from virtex_b200.factories import LRSchedulerFactory, OptimizerFactory, PretrainingModelFactory
     from virtex_b200.trainer import Trainer

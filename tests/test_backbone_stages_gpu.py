@@ -57,9 +57,8 @@ import torch
 from oracle import virtex_oracle as O
 from tests import backbone_replica as R
 from tests import backbone_stages as S
-from tests import basic_oracle as BO
 from tests import gemm_reference as G
-from tests import wide_oracle as WO
+from tests.helpers import build_model
 
 pytestmark = pytest.mark.gpu
 
@@ -555,22 +554,8 @@ def eng_sms():
 
 
 def _model(backbone, seed):
-    from virtex_b200.models import VirTexModel
-    from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    if backbone in BO.BLOCKS:
-        spec = BO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
-        state = BO.synth_state(spec, seed, residual_gain=0.25)
-    else:
-        spec = WO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
-        state = WO.synth_state(spec, seed, bn3_gain=0.25)
-    visual = TorchvisionVisualBackbone(backbone, visual_feature_size=spec.visual_feature_size)
-    textual = TransformerDecoderTextualHead(
-        visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
-        num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=0.0,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad)
-    model = VirTexModel(visual, textual)
-    model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
-    return model.cuda().train()
+    spec = O.Spec(backbone=backbone, hidden=128, layers=1, heads=2, ffn=256)
+    return build_model(spec, O.synth_state(spec, seed, bn3_gain=0.25)).train()
 
 
 CASES = [  # backbone, B, (H, W), fuse_bn3_min_rows (None: default), dynamic schedule, eval replay, weight-gradient

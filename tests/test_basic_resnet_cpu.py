@@ -10,7 +10,6 @@ import torchvision
 from torch import nn
 
 from oracle import virtex_oracle as O
-from tests import basic_oracle as BO
 from tests.test_engine_dryrun import _check_gemm, _model, _run
 
 BF16 = torch.bfloat16
@@ -83,8 +82,8 @@ def test_config_factory_and_optimizer_groups(name):
     model = PretrainingModelFactory.from_config(cfg)
     assert tuple(model.visual.cnn.layer2[0].conv1.weight.shape) == (128, 64, 3, 3)
     assert tuple(model.textual.visual_projection.weight.shape) == (1024, 512)
-    spec = BO.spec(name)
-    state = BO.synth_state(spec, 0)
+    spec = O.Spec(backbone=name)
+    state = O.synth_state(spec, 0)
     model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
     assert torch.equal(model.visual.cnn.layer4[0].conv1.weight, state["visual.cnn.layer4.0.conv1.weight"])
     named = list(model.named_parameters())
@@ -101,16 +100,16 @@ def test_config_factory_and_optimizer_groups(name):
 # ------------------------------------------------------------------------------------------ oracle vs the reference
 def _load(golden_dir):
     g = torch.load(os.path.join(golden_dir, "r18_l1_h128_post_b2.pt"), weights_only=False)
-    spec = BO.spec(**g["spec"])
+    spec = O.Spec(**g["spec"])
     batch = O.synth_batch(max_len=spec.max_len, vocab=spec.vocab, **g["batch"])
-    return g, spec, BO.synth_state(spec, g["seed"]), batch
+    return g, spec, O.synth_state(spec, g["seed"]), batch
 
 
 def test_oracle_train_forward_backward_f64(golden_dir):
     """float64 oracle == float64 reference VirTexModel with TorchvisionVisualBackbone("resnet18", 512)."""
     g, spec, state, batch = _load(golden_dir)
     assert spec.backbone == "resnet18"
-    out, grads, bufs = BO.loss_and_grads(state, batch, spec, dtype=torch.float64)
+    out, grads, bufs = O.loss_and_grads(state, batch, spec, dtype=torch.float64)
     ref = g["f64"]
     assert abs(out["loss"].item() - ref["loss"].item()) < 1e-9
     assert abs(out["loss_components"]["captioning_forward"].item() - ref["loss_forward"].item()) < 1e-9
@@ -130,7 +129,7 @@ def test_oracle_train_forward_backward_f64(golden_dir):
 def test_oracle_train_loss_f32(golden_dir):
     g, spec, state, batch = _load(golden_dir)
     with torch.no_grad():
-        out = BO.model_forward(state, batch, spec, training=True)
+        out = O.model_forward(state, batch, spec, training=True)
     for tag in ("f32", "f64"):
         assert abs(out["loss"].item() - g[tag]["loss"].item()) < 2e-6 * g[tag]["loss"].item()
 
@@ -140,8 +139,8 @@ def test_oracle_eval_logits_and_argmax(golden_dir):
     st64 = O.cast_state(state, torch.float64)
     b64 = dict(batch, image=batch["image"].double())
     with torch.no_grad():
-        out = BO.model_forward(st64, b64, spec, training=False, return_logits=True)
-        out32 = BO.model_forward(state, batch, spec, training=False)
+        out = O.model_forward(st64, b64, spec, training=False, return_logits=True)
+        out32 = O.model_forward(state, batch, spec, training=False)
     ref = g["f64"]
     assert out["visual_features"].shape[1] == 512
     assert abs(out["loss"].item() - ref["eval_loss"].item()) < 1e-9
@@ -152,25 +151,10 @@ def test_oracle_eval_logits_and_argmax(golden_dir):
     assert torch.equal(out32["predictions"], g["f32"]["eval_predictions"])
 
 
-@pytest.mark.parametrize("backbone", ["resnet18", "resnet34"])
-def test_oracle_backbone_shapes_are_torchvisions(backbone):
-    shapes = BO.backbone_param_shapes(BO.spec(backbone))
-    tv = _tv_backbone_sd(backbone)
-    assert list(shapes) == ["visual.cnn." + k for k in tv]
-    assert {k[len("visual.cnn."):]: v for k, v in shapes.items()} == {k: tuple(v.shape) for k, v in tv.items()}
-
-
-def test_basic_oracle_is_the_oracle_for_bottlenecks():
-    spec = O.Spec(hidden=128, layers=1, heads=2, ffn=256)
-    a, b = BO.synth_state(spec, 3, residual_gain=0.25), O.synth_state(spec, 3, bn3_gain=0.25)
-    assert list(a) == list(b) and all(torch.equal(a[k], b[k]) for k in a)
-    assert BO.backbone_forward.__module__ == "tests.basic_oracle" and O.backbone_forward is BO._BOTTLENECK_FORWARD
-
-
 def test_basic_synth_state_covers_the_reference_key_set():
-    spec = BO.spec("resnet34", hidden=128, layers=1, heads=2, ffn=256)
-    state = BO.synth_state(spec, 0, residual_gain=0.25)
-    shapes = {**BO.backbone_param_shapes(spec), **O.head_param_shapes(spec)}
+    spec = O.Spec(backbone="resnet34", hidden=128, layers=1, heads=2, ffn=256)
+    state = O.synth_state(spec, 0, bn3_gain=0.25)
+    shapes = {**O.backbone_param_shapes(spec), **O.head_param_shapes(spec)}
     assert list(state) == list(shapes) and all(tuple(state[k].shape) == shapes[k] for k in state)
     assert shapes["textual.visual_projection.weight"] == (128, 512)
     assert float(state["visual.cnn.layer1.0.bn2.weight"].max()) <= 1.5 * 0.25
@@ -220,7 +204,7 @@ def test_engine_schedule_of_a_basic_block_model(basic_dry, monkeypatch, backbone
     from virtex_b200.engine import Engine
     if fuse:  # the previous block's bn2 sums in every identity block's conv1 dgrad
         monkeypatch.setattr(Engine, "fuse_bn3_min_rows", 0)
-    spec = BO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
+    spec = O.Spec(backbone=backbone, hidden=128, layers=1, heads=2, ffn=256)
     model = _model(spec)
     batch = O.synth_batch(2, seed=0)
     eng = _run(model, batch)               # training forward + backward

@@ -11,7 +11,7 @@ GEMM checked against tests/gemm_reference.py: bounded on the real operands, then
 output must match bit for bit (the checker of tests/test_gemm_engine_gpu.py), once without and once with the bn2-sum
 fusion in every identity block.
 
-Then the backbone and the model against the float64 oracle of tests/basic_oracle.py with the bounds of
+Then the backbone and the model against the float64 oracle of oracle/virtex_oracle.py with the bounds of
 tests/test_wide_resnet_gpu.py, the model against the reference's fixture, the downstream forward against torchvision's
 resnet18 / resnet34 in float64, six Trainer steps, a beam search, and batch-256 steps of R18-L1-H1024 and R34-L1-H1024.
 
@@ -26,13 +26,14 @@ import torch
 from torch import nn
 
 from oracle import virtex_oracle as O
-from tests import basic_oracle as BO
 from tests import gemm_reference as G
+from tests.helpers import build_model, to_cuda
 
 pytestmark = pytest.mark.gpu
 
 F32 = torch.float32
-SMALL = BO.spec("resnet18", hidden=128, layers=1, heads=2, ffn=256)  # the spec of tests/golden/r18_l1_h128_post_b2.pt
+# the spec of tests/golden/r18_l1_h128_post_b2.pt
+SMALL = O.Spec(backbone="resnet18", hidden=128, layers=1, heads=2, ffn=256)
 
 
 def _ops():
@@ -50,23 +51,6 @@ def rel(a, b):
 def cos(a, b):
     a, b = a.detach().double().cpu().flatten(), b.detach().double().cpu().flatten()
     return (a @ b / (a.norm() * b.norm() + 1e-30)).item()
-
-
-def _build_model(spec, state, dropout=0.0):
-    from virtex_b200.models import VirTexModel
-    from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    visual = TorchvisionVisualBackbone(spec.backbone, visual_feature_size=spec.visual_feature_size)
-    textual = TransformerDecoderTextualHead(
-        visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
-        num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=dropout,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad)
-    model = VirTexModel(visual, textual)
-    model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
-    return model.cuda()
-
-
-def _to_cuda(batch):
-    return {k: v.cuda() for k, v in batch.items()}
 
 
 # ------------------------------------------------------------------------------------------ every GEMM, bit-exact
@@ -101,9 +85,9 @@ def test_engine_gemms_vs_reference(monkeypatch, backbone, fuse):
                          rmask=c.residual_mask is not None, bmask=c.bnr_mask is not None, view=c.out_view is not None))
 
     monkeypatch.setattr(E, "gemm", checked)
-    spec = BO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
-    model = _build_model(spec, BO.synth_state(spec, 2, residual_gain=0.25))
-    batch = _to_cuda(O.synth_batch(2, seed=4, ragged=True))
+    spec = O.Spec(backbone=backbone, hidden=128, layers=1, heads=2, ffn=256)
+    model = build_model(spec, O.synth_state(spec, 2, bn3_gain=0.25))
+    batch = to_cuda(O.synth_batch(2, seed=4, ragged=True))
     model.train()
     out = model(batch)
     out["loss"].backward()
@@ -129,9 +113,9 @@ def test_engine_gemms_vs_reference(monkeypatch, backbone, fuse):
 def test_backbone_forward_backward_vs_oracle(backbone):
     """tests/test_wide_resnet_gpu.py::test_backbone_forward_backward_vs_oracle on the basic-block backbones."""
     _ops()
-    spec = BO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
-    state = BO.synth_state(spec, 5, residual_gain=0.25)
-    model = _build_model(spec, state)
+    spec = O.Spec(backbone=backbone, hidden=128, layers=1, heads=2, ffn=256)
+    state = O.synth_state(spec, 5, bn3_gain=0.25)
+    model = build_model(spec, state)
     B = 4
     batch = O.synth_batch(B, seed=3)
     eng = model.engine
@@ -140,7 +124,7 @@ def test_backbone_forward_backward_vs_oracle(backbone):
     P = {k: (v.clone().requires_grad_(True) if not O.is_buffer(k) else v.clone()) for k, v in state.items()}
     nb = {}
     rec = {}
-    ref = BO.backbone_forward(P, batch["image"], spec, training=True, new_buffers=nb, record=rec, emulate_bf16=True)
+    ref = O.backbone_forward(P, batch["image"], spec, training=True, new_buffers=nb, record=rec, emulate_bf16=True)
     ref_nhwc = ref.permute(0, 2, 3, 1).reshape(B * h * w, -1)
     assert ref_nhwc.shape[1] == 512
     # stage by stage: every block's conv outputs and block output against the bf16-placement oracle
@@ -150,7 +134,7 @@ def test_backbone_forward_backward_vs_oracle(backbone):
             want = rec[q + key].permute(0, 2, 3, 1).reshape(r[key].shape)
             assert rel(r[key], want) < 5e-2, (q + key, rel(r[key], want))
     with torch.no_grad():
-        ref32 = BO.backbone_forward(state, batch["image"], spec, training=True)
+        ref32 = O.backbone_forward(state, batch["image"], spec, training=True)
     f_emul, f_32 = rel(feat, ref_nhwc), rel(feat, ref32.permute(0, 2, 3, 1).reshape(B * h * w, -1))
     dfeat = (torch.randn(ref_nhwc.shape, generator=torch.Generator().manual_seed(0)) * 0.01).bfloat16().float()
     ref_nhwc.backward(dfeat)
@@ -176,12 +160,12 @@ def test_backbone_forward_backward_vs_oracle(backbone):
 def test_model_loss_grads_and_folded_eval_vs_oracle():
     _ops()
     spec = SMALL
-    state = BO.synth_state(spec, 11, residual_gain=0.25)
-    model = _build_model(spec, state)
+    state = O.synth_state(spec, 11, bn3_gain=0.25)
+    model = build_model(spec, state)
     model.train()
     batch = O.synth_batch(4, seed=6, ragged=True)
-    out = model(_to_cuda(batch))
-    ref, grads, _ = BO.loss_and_grads(state, batch, spec)
+    out = model(to_cuda(batch))
+    ref, grads, _ = O.loss_and_grads(state, batch, spec)
     assert abs(out["loss"].item() - ref["loss"].item()) < 1e-3 * ref["loss"].item(), (out["loss"].item(), ref["loss"].item())
     out["loss"].backward()
     named = dict(model.named_parameters())
@@ -195,7 +179,7 @@ def test_model_loss_grads_and_folded_eval_vs_oracle():
     eng = model.engine
     image = batch["image"].cuda()
     with torch.no_grad():
-        ref_e = BO.model_forward(state, batch, spec, training=False, return_logits=True)
+        ref_e = O.model_forward(state, batch, spec, training=False, return_logits=True)
         feat, h, w = eng.backbone_infer(image)
         B = image.shape[0]
         mem = eng.visual_projection_forward(feat, B * h * w)
@@ -223,10 +207,10 @@ def test_model_vs_reference_fixture(golden_dir):
     residual gain 1): the training loss, and the eval loss and confident predictions."""
     _ops()
     g = torch.load(os.path.join(golden_dir, "r18_l1_h128_post_b2.pt"), weights_only=False)
-    spec = BO.spec(**g["spec"])
-    state = BO.synth_state(spec, g["seed"])
-    batch = _to_cuda(O.synth_batch(max_len=spec.max_len, vocab=spec.vocab, **g["batch"]))
-    model = _build_model(spec, state)
+    spec = O.Spec(**g["spec"])
+    state = O.synth_state(spec, g["seed"])
+    batch = to_cuda(O.synth_batch(max_len=spec.max_len, vocab=spec.vocab, **g["batch"]))
+    model = build_model(spec, state)
     model.train()
     with torch.no_grad():
         loss = model(batch)["loss"].item()
@@ -249,7 +233,7 @@ def test_downstream_forward_vs_torchvision_float64(name):
     _ops()
     import torchvision
     from virtex_b200.modules import ResNetParams
-    full = BO.synth_state(BO.spec(name), 41, residual_gain=0.25)
+    full = O.synth_state(O.Spec(backbone=name), 41, bn3_gain=0.25)
     state = {k[len("visual.cnn."):]: v for k, v in full.items() if k.startswith("visual.cnn.")}
     g = torch.Generator().manual_seed(42)
     state["fc.weight"] = torch.randn(10, 512, generator=g) * 0.05
@@ -282,18 +266,18 @@ def test_trainer_trajectory_vs_oracle():
     from virtex_b200.config import Config
     from virtex_b200.trainer import Trainer
     spec = SMALL
-    state = BO.synth_state(spec, 3, residual_gain=0.25)
-    model = _build_model(spec, state)
+    state = O.synth_state(spec, 3, bn3_gain=0.25)
+    model = build_model(spec, state)
     model.train()
     cfg = Config(None, ["MODEL.VISUAL.NAME", "torchvision::resnet18", "MODEL.VISUAL.FEATURE_SIZE", 512,
                         "MODEL.TEXTUAL.NAME", "transdec_postnorm::L1_H128_A2_F256", "MODEL.TEXTUAL.DROPOUT", 0.0,
                         "OPTIM.WARMUP_STEPS", 3, "OPTIM.NUM_ITERATIONS", 20, "OPTIM.BATCH_SIZE", 4,
                         "OPTIM.CNN_LR", 0.005])
     tr = Trainer(model, cfg)
-    ora = BO.OracleTrainer(state, spec, O.OptimCfg(warmup_steps=3, num_iterations=20, cnn_lr=0.005))
+    ora = O.OracleTrainer(state, spec, O.OptimCfg(warmup_steps=3, num_iterations=20, cnn_lr=0.005))
     for it in range(6):
         batch = O.synth_batch(4, seed=30 + it, ragged=True)
-        loss = tr.step(_to_cuda(batch)).sum().item()
+        loss = tr.step(to_cuda(batch)).sum().item()
         ref = ora.step(batch)
         print(f"r18 trainer step {it}: loss {loss:.6f} vs {ref['loss'].item():.6f}, grad norm "
               f"{tr.grad_norm.item():.4f} vs {ref['grad_norm'].item():.4f}")
@@ -331,13 +315,13 @@ def test_beam_search_on_resnet18():
 
 # ------------------------------------------------------------------------------------------------------ full size
 def _fp32_oracle(state, batch, spec, training):
-    """BO.model_forward in fp32 with the backbone evaluated on the GPU (TF32 off) and the head on the CPU."""
+    """O.model_forward in fp32 with the backbone evaluated on the GPU (TF32 off) and the head on the CPU."""
     flags = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
     try:
         P = {k: v.cuda() for k, v in state.items()}
         with torch.no_grad():
-            vf = BO.backbone_forward(P, batch["image"].cuda(), spec, training=training).cpu()
+            vf = O.backbone_forward(P, batch["image"].cuda(), spec, training=training).cpu()
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = flags
     with torch.no_grad():
@@ -353,12 +337,12 @@ def test_full_size_batch_256(backbone):
     of tests/test_wide_resnet_gpu.py, and a training step with finite gradients."""
     _ops()
     torch.set_num_threads(max(1, min(32, (torch.get_num_threads() or 1))))
-    spec = BO.spec(backbone)
-    state = BO.synth_state(spec, 23, residual_gain=0.25)
-    model = _build_model(spec, state)
+    spec = O.Spec(backbone=backbone)
+    state = O.synth_state(spec, 23, bn3_gain=0.25)
+    model = build_model(spec, state)
     B = 256
     batch = O.synth_batch(B, seed=31, ragged=True)
-    cb = _to_cuda(batch)
+    cb = to_cuda(batch)
     torch.cuda.reset_peak_memory_stats()
     model.train()
     with torch.no_grad():

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from tests import classification_oracle as CO
+from tests.helpers import to_cuda
 
 pytestmark = pytest.mark.gpu
 BF16 = torch.bfloat16
@@ -150,10 +151,6 @@ def _model(name, frozen=False):
     return model.cuda().train(), state, vocab, ignore, batch_seed
 
 
-def _cuda(batch):
-    return {k: v.cuda() for k, v in batch.items()}
-
-
 @pytest.mark.parametrize("name", list(CO.CASES))
 @pytest.mark.parametrize("frozen", [False, True])
 def test_classification_model_vs_oracle(name, frozen):
@@ -162,7 +159,7 @@ def test_classification_model_vs_oracle(name, frozen):
     _need_cuda()
     model, state, vocab, ignore, batch_seed = _model(name, frozen)
     batch = CO.synth_label_batch(6, seed=batch_seed, vocab=vocab, ignore=ignore, image_size=224)
-    out = model(_cuda(batch))
+    out = model(to_cuda(batch))
     ref, grads = CO.loss_and_grads(state, batch, ignore, torch.float64)
     assert set(out["loss_components"]) == {"classification"}
     assert abs(out["loss"].item() - ref["loss"].item()) < 1e-3 * ref["loss"].item(), (out["loss"].item(), ref["loss"].item())
@@ -180,7 +177,7 @@ def test_classification_model_vs_oracle(name, frozen):
     model.load_state_dict(state, strict=True)  # the BN running statistics the oracle's eval pass uses
     model.eval()
     with torch.no_grad():
-        ev = model(_cuda(batch))
+        ev = model(to_cuda(batch))
     ref_ev = CO.eval_forward(state, batch, ignore, torch.float64)
     assert abs(ev["loss"].item() - ref_ev["loss"].item()) < 2e-3 * ref_ev["loss"].item()
     pred = ev["predictions"].cpu()
@@ -206,7 +203,7 @@ def test_empty_label_set_on_the_engine():
     model, state, vocab, ignore, batch_seed = _model("multilabel_classification")
     batch = CO.synth_label_batch(3, seed=batch_seed, vocab=vocab, ignore=ignore, image_size=224,
                                  empty_rows=(CO.EMPTY_ROW,))
-    out = model(_cuda(batch))
+    out = model(to_cuda(batch))
     assert torch.isnan(out["loss"])
     out["loss"].backward()
     _, grads = CO.loss_and_grads(state, batch, ignore, torch.float64)
@@ -235,7 +232,8 @@ def test_trainer_steps_match_the_autograd_loop():
     opt = OptimizerFactory.from_config(cfg, ref.named_parameters())
     sched = LRSchedulerFactory.from_config(cfg, opt)
     for it in range(3):
-        batch = _cuda(CO.synth_label_batch(4, seed=60 + it, vocab=10000, ignore=CO.TOKEN_IGNORE, image_size=224))
+        batch = to_cuda(CO.synth_label_batch(4, seed=60 + it, vocab=10000, ignore=CO.TOKEN_IGNORE,
+                                             image_size=224))
         loss = trainer.step(batch)
         opt.zero_grad()
         out = ref(batch)

@@ -20,6 +20,7 @@ import pytest
 import torch
 
 from oracle import virtex_oracle as O
+from tests.helpers import build_model, to_cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -37,24 +38,6 @@ def rel(a, b):
 def cos(a, b):
     a, b = a.detach().float().cpu().flatten(), b.detach().float().cpu().flatten()
     return (a @ b / (a.norm() * b.norm() + 1e-30)).item()
-
-
-def build_model(spec: O.Spec, state, dropout=0.0):
-    from virtex_b200.models import VirTexModel
-    from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    visual = TorchvisionVisualBackbone(spec.backbone, visual_feature_size=spec.visual_feature_size)
-    textual = TransformerDecoderTextualHead(
-        visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
-        num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=dropout,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad,
-        mask_future_positions=spec.mask_future)
-    model = VirTexModel(visual, textual)
-    missing = model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
-    return model.cuda()
-
-
-def to_cuda(batch):
-    return {k: v.cuda() for k, v in batch.items()}
 
 
 # ----------------------------------------------------------------------------------------------------------- kernels

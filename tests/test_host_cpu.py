@@ -7,24 +7,14 @@ import pytest
 import torch
 
 from oracle import virtex_oracle as O
+from tests.helpers import virtex_model
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _build(spec):
-    from virtex_b200.models import VirTexModel
-    from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    visual = TorchvisionVisualBackbone(spec.backbone, visual_feature_size=spec.visual_feature_size)
-    textual = TransformerDecoderTextualHead(
-        visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
-        num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=0.1,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad)
-    return VirTexModel(visual, textual)
-
-
 def test_state_dict_matches_reference_key_set():
     spec = O.Spec()
-    model = _build(spec)
+    model = virtex_model(spec, dropout=0.1)
     ref_sd = O.to_reference_state_dict(O.synth_state(spec, 0), spec)
     sd = model.state_dict()
     assert set(sd) == set(ref_sd)
@@ -38,7 +28,7 @@ def test_state_dict_matches_reference_key_set():
 
 def test_weight_sharing_and_init():
     spec = O.Spec(hidden=128, layers=2, heads=2, ffn=256)
-    m = _build(spec)
+    m = virtex_model(spec, dropout=0.1)
     assert m.backward_textual.embedding is m.textual.embedding
     assert m.backward_textual.visual_projection is m.textual.visual_projection
     assert m.backward_textual.output is m.textual.output
@@ -52,7 +42,7 @@ def test_weight_sharing_and_init():
 
 def test_no_cpu_fallback():
     spec = O.Spec(hidden=128, layers=1, heads=2, ffn=256)
-    m = _build(spec)
+    m = virtex_model(spec, dropout=0.1)
     batch = O.synth_batch(2, 0)
     with pytest.raises(RuntimeError, match="no CPU path"):
         m(batch)

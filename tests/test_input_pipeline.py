@@ -130,7 +130,7 @@ def test_gpu_val_transform_and_model_consumes_the_batch():
         assert np.array_equal(out[n], P.val_transform(im)), n
     # the batch dict is what CaptioningModel.forward takes (captioning.py:71-77)
     from oracle import virtex_oracle as O
-    from tests.test_gpu_parity import build_model
+    from tests.helpers import build_model
     spec = O.Spec(hidden=128, layers=1, heads=2, ffn=256)
     model = build_model(spec, O.synth_state(spec, 3, bn3_gain=0.25)).eval()
     del batch["_image_u8"]

@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "jpeg_decode.npz")
 
 
-def _cuda():
+def _need_cuda():
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
 
@@ -44,7 +44,7 @@ def _on_device(items):
 
 
 def test_decode_is_bit_exact_on_the_golden_corpus():
-    _cuda()
+    _need_cuda()
     from virtex_b200 import jpeg
     items = _on_device(_golden())
     out = jpeg.decode([g["buf"] for g in items], "cuda")
@@ -55,7 +55,7 @@ def test_decode_is_bit_exact_on_the_golden_corpus():
 
 
 def test_batch_of_256_mixed_sizes():
-    _cuda()
+    _need_cuda()
     from virtex_b200 import jpeg
     items = _on_device(_golden())
     large = [g for g in items if g["name"].startswith("large")]
@@ -74,7 +74,7 @@ def test_batch_of_256_mixed_sizes():
 @pytest.mark.parametrize("chunk_bits", ["shorter", "exact", 64, 256])
 def test_segment_lengths_against_the_chunk_size(chunk_bits):
     """One chunk longer than the segment, exactly one chunk, and many chunks per segment."""
-    _cuda()
+    _need_cuda()
     from virtex_b200 import jpeg
     items = {g["name"]: g for g in _golden()}
     names = ["gray_q90_rst0_1x1", "420_q90_37x53", "444_q75_rst1_29x45", "large_480x640_q90_422_rst8"]
@@ -95,7 +95,7 @@ def test_segment_lengths_against_the_chunk_size(chunk_bits):
 
 
 def test_pipeline_fed_jpeg_bytes_equals_the_pipeline_fed_decoded_arrays():
-    _cuda()
+    _need_cuda()
     pytest.importorskip("cv2")  # the progressive / CMYK / truncated items are decoded by cv2
     from virtex_b200 import jpeg
     from virtex_b200.data_gpu import GpuInputPipeline
@@ -137,7 +137,7 @@ def test_pipeline_fed_jpeg_bytes_equals_the_pipeline_fed_decoded_arrays():
 
 
 def test_corrupt_entropy_data_falls_back_to_cv2_and_the_next_call_works():
-    _cuda()
+    _need_cuda()
     pytest.importorskip("cv2")
     from virtex_b200 import jpeg
     g = {x["name"]: x for x in _golden()}

@@ -21,6 +21,7 @@ from oracle import virtex_oracle as O
 from tests import attention_replica as AR
 from tests import dropout_replica as R
 from tests import head_stages as S
+from tests.helpers import build_model, to_cuda
 from tests.test_head_kernels_gpu import _allowed, _flip_floor, _heads, _rb, assert_bf16, assert_f32, rel
 
 pytestmark = pytest.mark.gpu
@@ -283,23 +284,6 @@ def test_head_stages_replay_at_100_keys(H, L, A, Fd, norm_first, task, B, T, mon
 
 
 # ------------------------------------------------------------------------------------------------ whole model
-def _build(spec, state, dropout=0.0):
-    from virtex_b200.models import VirTexModel
-    from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    visual = TorchvisionVisualBackbone(spec.backbone, visual_feature_size=spec.visual_feature_size)
-    textual = TransformerDecoderTextualHead(
-        visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
-        num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=dropout,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad)
-    model = VirTexModel(visual, textual)
-    model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
-    return model.cuda()
-
-
-def _cuda(batch):
-    return {k: v.cuda() for k, v in batch.items()}
-
-
 def _cos(a, b):
     a, b = a.detach().double().cpu().flatten(), b.detach().double().cpu().flatten()
     return (a @ b / (a.norm() * b.norm() + 1e-30)).item()
@@ -320,10 +304,10 @@ def test_model_at_crop_288_and_40_tokens_vs_oracle():
     _need_cuda()
     spec = O.Spec(**SPEC_288)
     state = O.synth_state(spec, 11, bn3_gain=0.25)
-    model = _build(spec, state)
+    model = build_model(spec, state)
     model.train()
     batch = O.synth_batch(4, seed=6, ragged=True, max_len=40, image_size=288)
-    out = model(_cuda(batch))
+    out = model(to_cuda(batch))
     ref, grads, _ = O.loss_and_grads(state, batch, spec)
     assert abs(out["loss"].item() - ref["loss"].item()) < 1e-3 * ref["loss"].item(), (out["loss"].item(),
                                                                                       ref["loss"].item())
@@ -334,7 +318,7 @@ def test_model_at_crop_288_and_40_tokens_vs_oracle():
     assert not bad, bad
     model.eval()
     with torch.no_grad():
-        out = model(_cuda(batch))
+        out = model(to_cuda(batch))
         ref = O.model_forward(state, batch, spec, training=False, return_logits=True)
     assert abs(out["loss"].item() - ref["loss"].item()) < 2e-3 * ref["loss"].item()
     pred, pref = out["predictions"].cpu(), ref["predictions"]
@@ -355,12 +339,12 @@ def test_trainer_step_at_crop_288_and_40_tokens_vs_autograd():
                         "DATA.IMAGE_CROP_SIZE", 288, "DATA.MAX_CAPTION_LENGTH", 40, "OPTIM.WARMUP_STEPS", 0,
                         "OPTIM.NUM_ITERATIONS", 100, "OPTIM.BATCH_SIZE", 4])
     state = O.synth_state(spec, 3, bn3_gain=0.25)
-    model, twin = _build(spec, state).train(), _build(spec, state).train()
+    model, twin = build_model(spec, state).train(), build_model(spec, state).train()
     trainer = Trainer(model, cfg)
     opt = OptimizerFactory.from_config(cfg, twin.named_parameters())
     sched = LRSchedulerFactory.from_config(cfg, opt)
     for it in range(2):
-        batch = _cuda(O.synth_batch(4, seed=30 + it, ragged=True, max_len=40, image_size=288))
+        batch = to_cuda(O.synth_batch(4, seed=30 + it, ragged=True, max_len=40, image_size=288))
         loss = trainer.step(batch).sum().item()
         opt.zero_grad()
         out = twin(batch)

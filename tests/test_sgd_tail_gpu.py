@@ -15,7 +15,6 @@ import pytest
 import torch
 
 from oracle import virtex_oracle as O
-from tests import basic_oracle as BO
 from tests import classification_oracle as CO
 from tests import sgd_tail as T
 
@@ -206,7 +205,7 @@ def test_nan_gradient_norm_makes_every_updated_parameter_nan(optimizer):
 # ------------------------------------------------------------------------------------------------------------- models
 _HEAD = ["MODEL.TEXTUAL.NAME", "transdec_postnorm::L1_H128_A2_F256", "MODEL.TEXTUAL.DROPOUT", 0.0]
 _R50 = O.Spec(hidden=128, layers=1, heads=2, ffn=256)
-_R18 = BO.spec("resnet18", hidden=128, layers=1, heads=2, ffn=256)
+_R18 = O.Spec(backbone="resnet18", hidden=128, layers=1, heads=2, ffn=256)
 _ONE_WAY = {"captioning": O.Spec(hidden=128, layers=1, heads=2, ffn=256, caption_backward=False),
             "masked_lm": O.Spec(hidden=128, layers=1, heads=2, ffn=256, caption_backward=False, mask_future=False)}
 
@@ -250,7 +249,7 @@ def _model(kind, *extra):
         spec = _R18 if r18 else _R50
         cfg = Config(None, _HEAD + (["MODEL.VISUAL.NAME", "torchvision::resnet18", "MODEL.VISUAL.FEATURE_SIZE", 512]
                                     if r18 else []) + list(extra))
-        state = BO.synth_state(spec, 7, residual_gain=0.25) if r18 else O.synth_state(spec, 7, bn3_gain=0.25)
+        state = O.synth_state(spec, 7, bn3_gain=0.25)
         sd = O.to_reference_state_dict(state, spec)
 
         def batch(seed, B=4):

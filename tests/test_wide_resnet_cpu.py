@@ -1,7 +1,8 @@
 """Wide ResNet-50-2 / 101-2 backbones (the reference's R_50W2X ablation, `torchvision::wide_resnet50_2`) on the CPU:
 the parameter tree against torchvision's, the shipped config and the factories, the float64 oracle against the
 reference's own VirTexModel (tests/golden/r50w2x_l1_h128_post_b2.pt, written by scripts/make_wide_golden.py), and a dry run
-of the engine's schedule for a wide model."""
+of the engine's schedule for a wide model.  The oracle's parameter inventory is checked here against torchvision's for
+every ResNet it states, basic-block ones included."""
 import os
 
 import pytest
@@ -10,7 +11,6 @@ import torchvision
 from torch import nn
 
 from oracle import virtex_oracle as O
-from tests import wide_oracle as WO
 from tests.test_engine_dryrun import _check_gemm, _model, _run
 
 
@@ -66,8 +66,8 @@ def test_config_factory_and_optimizer_groups():
     model = PretrainingModelFactory.from_config(cfg)
     assert tuple(model.visual.cnn.layer2[0].conv2.weight.shape) == (256, 256, 3, 3)
     # a reference checkpoint of this config (TorchvisionVisualBackbone("wide_resnet50_2")) loads strictly
-    spec = WO.spec("wide_resnet50_2")
-    state = WO.synth_state(spec, 0)
+    spec = O.Spec(backbone="wide_resnet50_2")
+    state = O.synth_state(spec, 0)
     model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
     assert torch.equal(model.visual.cnn.layer4[0].conv2.weight, state["visual.cnn.layer4.0.conv2.weight"])
     named = list(model.named_parameters())
@@ -81,9 +81,9 @@ def test_config_factory_and_optimizer_groups():
 # ------------------------------------------------------------------------------------------ oracle vs the reference
 def _load(golden_dir):
     g = torch.load(os.path.join(golden_dir, "r50w2x_l1_h128_post_b2.pt"), weights_only=False)
-    spec = WO.spec(**g["spec"])
+    spec = O.Spec(**g["spec"])
     batch = O.synth_batch(max_len=spec.max_len, vocab=spec.vocab, **g["batch"])
-    return g, spec, WO.synth_state(spec, g["seed"]), batch
+    return g, spec, O.synth_state(spec, g["seed"]), batch
 
 
 def test_oracle_train_forward_backward_f64(golden_dir):
@@ -131,26 +131,18 @@ def test_oracle_eval_logits_and_argmax(golden_dir):
     assert torch.equal(out32["predictions"], g["f32"]["eval_predictions"])
 
 
-@pytest.mark.parametrize("backbone", ["resnet50", "resnet101", "resnet152", "wide_resnet50_2", "wide_resnet101_2"])
+@pytest.mark.parametrize("backbone", list(O._RESNET_LAYERS))
 def test_oracle_backbone_shapes_are_torchvisions(backbone):
-    shapes = WO.backbone_param_shapes(WO.spec(backbone))
+    shapes = O.backbone_param_shapes(O.Spec(backbone=backbone))
     tv = _tv_backbone_sd(backbone)
     assert list(shapes) == ["visual.cnn." + k for k in tv]
     assert {k[len("visual.cnn."):]: v for k, v in shapes.items()} == {k: tuple(v.shape) for k, v in tv.items()}
 
 
-@pytest.mark.parametrize("backbone", ["resnet50", "resnet101"])
-def test_wide_oracle_is_the_oracle_for_resnets(backbone):
-    spec = WO.spec(backbone, hidden=128, layers=1, heads=2, ffn=256)
-    assert WO.backbone_param_shapes(spec) == O.backbone_param_shapes(spec)
-    a, b = WO.synth_state(spec, 3, bn3_gain=0.25), O.synth_state(spec, 3, bn3_gain=0.25)
-    assert list(a) == list(b) and all(torch.equal(a[k], b[k]) for k in a)
-
-
 def test_wide_synth_state_covers_the_reference_key_set():
-    spec = WO.spec("wide_resnet50_2", hidden=128, layers=1, heads=2, ffn=256)
-    state = WO.synth_state(spec, 0, bn3_gain=0.25)
-    shapes = {**WO.backbone_param_shapes(spec), **O.head_param_shapes(spec)}
+    spec = O.Spec(backbone="wide_resnet50_2", hidden=128, layers=1, heads=2, ffn=256)
+    state = O.synth_state(spec, 0, bn3_gain=0.25)
+    shapes = {**O.backbone_param_shapes(spec), **O.head_param_shapes(spec)}
     assert list(state) == list(shapes) and all(tuple(state[k].shape) == shapes[k] for k in state)
     assert torch.equal(state["textual.embedding.words.weight"],
                        O.synth_state(O.Spec(hidden=128, layers=1, heads=2, ffn=256), 0)["textual.embedding.words.weight"])
@@ -182,7 +174,7 @@ def wide_dry(monkeypatch):
 
 
 def test_engine_schedule_of_a_wide_model(wide_dry):
-    spec = WO.spec("wide_resnet50_2", hidden=128, layers=1, heads=2, ffn=256)
+    spec = O.Spec(backbone="wide_resnet50_2", hidden=128, layers=1, heads=2, ffn=256)
     model = _model(spec)
     batch = O.synth_batch(2, seed=0)
     eng = _run(model, batch)               # training forward + backward

@@ -25,7 +25,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from oracle import virtex_oracle as O
-from tests import wide_oracle as WO
+from tests.helpers import build_model, to_cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -206,31 +206,14 @@ def test_conv3_fprop_dgrad_wgrad(H, C4, width):
 
 
 # ------------------------------------------------------------------------------------------------------- backbone
-def _build_model(spec, state, dropout=0.0):
-    from virtex_b200.models import VirTexModel
-    from virtex_b200.modules import TorchvisionVisualBackbone, TransformerDecoderTextualHead
-    visual = TorchvisionVisualBackbone(spec.backbone, visual_feature_size=spec.visual_feature_size)
-    textual = TransformerDecoderTextualHead(
-        visual_feature_size=spec.visual_feature_size, vocab_size=spec.vocab, hidden_size=spec.hidden,
-        num_layers=spec.layers, attention_heads=spec.heads, feedforward_size=spec.ffn, dropout=dropout,
-        norm_first=spec.norm_first, max_caption_length=spec.max_len, padding_idx=spec.pad)
-    model = VirTexModel(visual, textual)
-    model.load_state_dict(O.to_reference_state_dict(state, spec), strict=True)
-    return model.cuda()
-
-
-def _to_cuda(batch):
-    return {k: v.cuda() for k, v in batch.items()}
-
-
-SMALL = WO.spec(WIDE, hidden=128, layers=1, heads=2, ffn=256)  # the spec of tests/golden/r50w2x_*.pt
+SMALL = O.Spec(backbone=WIDE, hidden=128, layers=1, heads=2, ffn=256)  # the spec of tests/golden/r50w2x_*.pt
 
 
 def test_backbone_forward_backward_vs_oracle():
     """tests/test_gpu_parity.py::test_backbone_forward_backward_vs_oracle on the wide backbone, same bounds."""
     _ops()
-    state = WO.synth_state(SMALL, 5, bn3_gain=0.25)
-    model = _build_model(SMALL, state)
+    state = O.synth_state(SMALL, 5, bn3_gain=0.25)
+    model = build_model(SMALL, state)
     B = 4
     batch = O.synth_batch(B, seed=3)
     eng = model.engine
@@ -266,11 +249,11 @@ def test_backbone_forward_backward_vs_oracle():
 def test_model_loss_grads_and_folded_eval_vs_oracle():
     _ops()
     spec = SMALL
-    state = WO.synth_state(spec, 11, bn3_gain=0.25)
-    model = _build_model(spec, state)
+    state = O.synth_state(spec, 11, bn3_gain=0.25)
+    model = build_model(spec, state)
     model.train()
     batch = O.synth_batch(4, seed=6, ragged=True)
-    out = model(_to_cuda(batch))
+    out = model(to_cuda(batch))
     ref, grads, _ = O.loss_and_grads(state, batch, spec)
     assert abs(out["loss"].item() - ref["loss"].item()) < 1e-3 * ref["loss"].item(), (out["loss"].item(), ref["loss"].item())
     out["loss"].backward()
@@ -316,7 +299,7 @@ def test_downstream_forward_vs_torchvision_float64():
     _ops()
     import torchvision
     from virtex_b200.modules import ResNetParams
-    full = WO.synth_state(SMALL, 41, bn3_gain=0.25)
+    full = O.synth_state(SMALL, 41, bn3_gain=0.25)
     state = {k[len("visual.cnn."):]: v for k, v in full.items() if k.startswith("visual.cnn.")}
     g = torch.Generator().manual_seed(42)
     state["fc.weight"] = torch.randn(10, 2048, generator=g) * 0.01
@@ -349,8 +332,8 @@ def test_trainer_trajectory_vs_oracle():
     from virtex_b200.config import Config
     from virtex_b200.trainer import Trainer
     spec = SMALL
-    state = WO.synth_state(spec, 3, bn3_gain=0.25)
-    model = _build_model(spec, state)
+    state = O.synth_state(spec, 3, bn3_gain=0.25)
+    model = build_model(spec, state)
     model.train()
     cfg = Config(None, ["MODEL.VISUAL.NAME", "torchvision::" + WIDE, "MODEL.TEXTUAL.NAME",
                         "transdec_postnorm::L1_H128_A2_F256", "MODEL.TEXTUAL.DROPOUT", 0.0, "OPTIM.WARMUP_STEPS", 3,
@@ -359,7 +342,7 @@ def test_trainer_trajectory_vs_oracle():
     ora = O.OracleTrainer(state, spec, O.OptimCfg(warmup_steps=3, num_iterations=20, cnn_lr=0.005))
     for it in range(6):
         batch = O.synth_batch(4, seed=30 + it, ragged=True)
-        loss = tr.step(_to_cuda(batch)).sum().item()
+        loss = tr.step(to_cuda(batch)).sum().item()
         ref = ora.step(batch)
         print(f"wide trainer step {it}: loss {loss:.6f} vs {ref['loss'].item():.6f}, grad norm "
               f"{tr.grad_norm.item():.4f} vs {ref['grad_norm'].item():.4f}")
@@ -394,12 +377,12 @@ def test_full_size_r50w2x_batch_256():
     the eval argmax rule of test_full_size_forward_vs_oracle_batch_256, and a training step with finite gradients."""
     _ops()
     torch.set_num_threads(max(1, min(32, (torch.get_num_threads() or 1))))
-    spec = WO.spec(WIDE)
-    state = WO.synth_state(spec, 23, bn3_gain=0.25)
-    model = _build_model(spec, state)
+    spec = O.Spec(backbone=WIDE)
+    state = O.synth_state(spec, 23, bn3_gain=0.25)
+    model = build_model(spec, state)
     B = 256
     batch = O.synth_batch(B, seed=31, ragged=True)
-    cb = _to_cuda(batch)
+    cb = to_cuda(batch)
     torch.cuda.reset_peak_memory_stats()
     model.train()
     with torch.no_grad():
