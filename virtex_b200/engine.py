@@ -18,6 +18,7 @@ from __future__ import annotations
 
 import math
 import struct
+from collections import namedtuple
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -144,20 +145,32 @@ def _require_cuda(dev):
         raise RuntimeError("virtex_b200 has no CPU path: move the model to a CUDA device first (model.cuda())")
 
 
-def _block_widths(blk):
-    """(inner width of conv1 / conv2, output width of conv3) of a bottleneck, read from its weights: 4x apart for
-    ResNet-50/101/152, 2x for the wide models.  A basic block's two 3x3 convs and its output share one width."""
-    if isinstance(blk, BasicBlock):
-        return blk.conv1.weight.shape[0], blk.conv2.weight.shape[0]
-    return blk.conv1.weight.shape[0], blk.conv3.weight.shape[0]
+_Conv = namedtuple("_Conv", "w k stride cin cout")
 
 
-def _convs3x3(name, blk):
-    """(weight prefix, stride) of every 3x3 conv of block `name`: conv2 of a bottleneck; conv1 (strided) and conv2 of a
-    basic block."""
-    if isinstance(blk, BasicBlock):
-        return [(name + ".conv1", blk.stride), (name + ".conv2", 1)]
-    return [(name + ".conv2", blk.stride)]
+def _block_convs(name, blk):
+    """The main-branch convolutions of residual block `name`, in order, as _Conv(weight prefix, kernel size, stride,
+    Cin, Cout); BN i follows conv i, and the last BN is the block output's.  A bottleneck is 1x1, 3x3 (the block's
+    stride), 1x1, its widths read from the weights (4x apart for ResNet-50/101/152, 2x for the wide models); a basic
+    block is two 3x3 convs, the first strided."""
+    kinds = [(3, blk.stride), (3, 1)] if isinstance(blk, BasicBlock) else [(1, 1), (3, blk.stride), (1, 1)]
+    convs = []
+    for i, (k, stride) in enumerate(kinds, 1):
+        cout, cin = getattr(blk, f"conv{i}").weight.shape[:2]
+        convs.append(_Conv(f"{name}.conv{i}", k, stride, cin, cout))
+    return convs
+
+
+def _dgrad_route(conv, cols):
+    """How the input gradient of main-branch conv `conv` runs: 'gemm' (1x1), 'implicit' (3x3, stride 1), 'parity'
+    (3x3, stride 2: one implicit GEMM per parity class of the input position) or 'col2im' (per-tap gradients by a plain
+    GEMM, scattered back: after an im2col forward, whose matrix is `cols`, and at other strides).  Only the GEMMs that
+    write dx itself carry an epilogue over it; 'parity' carries only the BN-backward sums."""
+    if conv.k == 1:
+        return "gemm"
+    if cols is not None or conv.stride not in (1, 2):
+        return "col2im"
+    return "implicit" if conv.stride == 1 else "parity"
 
 
 def _transposed_wgrad(Cin, C, stride):
@@ -238,13 +251,11 @@ class Engine:
             layer = getattr(cnn, f"layer{li}")
             for bi, blk in enumerate(layer):
                 self.blocks.append((f"visual.cnn.layer{li}.{bi}", blk))
+        self._convs = {name: _block_convs(name, blk) for name, blk in self.blocks}
         # fp32 weight-gradient scratch of every k > 1 convolution (GEMM output layout), one flat buffer zeroed once per
         # backward; the batched unpack jobs fold it into the OIHW gradient arena per all-reduce bucket
         sizes = [("visual.cnn.conv1", 64 * 256)]
-        for name, blk in self.blocks:  # [C, 9 * Cin] per 3x3 conv: conv2, and a basic block's conv1
-            if isinstance(blk, BasicBlock):
-                sizes.append((name + ".conv1", blk.conv1.weight.numel()))
-            sizes.append((name + ".conv2", blk.conv2.weight.numel()))
+        sizes += [(c.w, c.cout * 9 * c.cin) for convs in self._convs.values() for c in convs if c.k == 3]
         total = sum(_round_up(n, _ALIGN) for _, n in sizes)
         self._dwp_flat = torch.zeros(total, dtype=F32, device=self.device)
         self._dwp, off = {}, 0
@@ -278,9 +289,10 @@ class Engine:
                 (w, self._pack_buf("visual.cnn.conv1.weight#s2d", (64, 256)), 64 * 256, 64, 3, 7, 7, 256, 4)]
         for name, blk in self.blocks:
             parity = []
-            for wname, stride in _convs3x3(name, blk):
+            for wname, k, stride, I, O in self._convs[name]:
+                if k == 1:
+                    continue
                 w = self.P(wname + ".weight")
-                O, I = w.shape[0], w.shape[1]
                 rows.append((w, self._pack_buf(wname + ".weight", (O, 9 * I)), 9 * O * I, O, I, 3, 3, 9 * I, 0))
                 if stride == 1:
                     rows.append((w, self._pack_buf(wname + ".weight#dgrad", (I, 9 * O)), 9 * O * I, O, I, 3, 3, 9 * O,
@@ -304,13 +316,13 @@ class Engine:
         """Unpack-accumulate jobs of one gradient bucket: 'layer4' / 'layer3' / 'layer2' / 'rest' (layer1 + stem)."""
         rows = []
         want = "layer1" if layer == "rest" else layer
-        for name, blk in self.blocks:
+        for name, _ in self.blocks:
             if name.split(".")[2] != want:
                 continue
-            for wname, stride in _convs3x3(name, blk):
-                O, I = self.G(wname + ".weight").shape[:2]
-                rows.append((self._dwp[wname], self.G(wname + ".weight"), 9 * O * I, O, I, 3, 3, 9 * I,
-                             3 if _transposed_wgrad(I, O, stride) else 2))
+            for wname, k, stride, I, O in self._convs[name]:
+                if k == 3:
+                    rows.append((self._dwp[wname], self.G(wname + ".weight"), 9 * O * I, O, I, 3, 3, 9 * I,
+                                 3 if _transposed_wgrad(I, O, stride) else 2))
         if layer == "rest":
             g = self.G("visual.cnn.conv1.weight")
             if stem_s2d:
@@ -336,12 +348,10 @@ class Engine:
         """(name, channels) of every BatchNorm of the backbone."""
         out = [("visual.cnn.bn1", 64)]
         for name, blk in self.blocks:
-            width, C4 = _block_widths(blk)
-            out += [(name + ".bn1", width), (name + ".bn2", width)]
-            if not isinstance(blk, BasicBlock):
-                out.append((name + ".bn3", C4))
+            convs = self._convs[name]
+            out += [(f"{name}.bn{i}", c.cout) for i, c in enumerate(convs, 1)]
             if blk.downsample is not None:
-                out.append((name + ".downsample.1", C4))
+                out.append((name + ".downsample.1", convs[-1].cout))
         return out
 
     def _pack_buf(self, key, shape):
@@ -374,11 +384,7 @@ class Engine:
 
     def _stats_slab(self, training):
         """One zeroed fp32 slab per step holding every BN's [2,C] sum/sumsq (fwd) and [2,C] dz sums (bwd)."""
-        total = 2 * 64 * 2
-        for name, blk in self.blocks:
-            width, C4 = _block_widths(blk)
-            bn3 = 0 if isinstance(blk, BasicBlock) else C4
-            total += 2 * 2 * (width + width + bn3 + (C4 if blk.downsample is not None else 0))
+        total = 4 * sum(C for _, C in self._bn_names())
         slab = self.ws.get("bn_slab", (total,), F32)
         slab.zero_()
         self._slab, self._slab_off = slab, 0
@@ -410,11 +416,15 @@ class Engine:
         gemm(cols, self._packed["visual.cnn.conv1.weight"], y0, M0, 64, 160, **epi)
         return None, cols
 
-    def _conv3x3(self, wname, x, y, B, Hc, Wc, stride, key, **epi):
-        """3x3 conv (stride 1 or 2, pad 1) whose weight is `wname`: x [B*Hc*Wc, Cin] -> y [Mout, C]; returns the
-        im2col matrix when that route ran, else None."""
-        Mout, C = y.shape
-        Cin = x.shape[1]
+    def _conv(self, conv, x, y, B, Hc, Wc, key, **epi):
+        """Main-branch conv `conv` (a _Conv) of a residual block: x [B*Hc*Wc, Cin] -> y [Mout, C]; a 1x1 conv is a plain
+        GEMM, a 3x3 conv (stride 1 or 2, pad 1) an implicit GEMM or im2col + GEMM.  Returns the im2col matrix when that
+        route ran, else None."""
+        wname, k, stride, Cin, C = conv
+        Mout = y.shape[0]
+        if k == 1:
+            gemm(x, self.W(wname + ".weight").view(C, Cin), y, Mout, C, Cin, **epi)
+            return None
         w = self._packed[wname + ".weight"]
         if Cin % 64 == 0:
             # implicit GEMM: 4-D TMA boxes gather the taps (zero fill = padding); stride 2 through TMA traversal strides
@@ -482,55 +492,36 @@ class Engine:
         call("vtx_bn_relu_maxpool", y0.data_ptr(), bnp0.data_ptr(), x.data_ptr(), idx.data_ptr(), B, Ho, Wo, 64, s)
         tape["stem"] = dict(cols=cols, s2d=s2d, y=y0, bnp=bnp0, idx=idx, Ho=Ho, Wo=Wo, Hp=Hp, Wp=Wp, M=M0)
         Hc, Wc, Cin = Hp, Wp, 64
-        # ---- residual blocks
+        # ---- residual blocks (torchvision's basic and bottleneck blocks): every conv but the last with statistics ->
+        # its BN + ReLU; the last with statistics -> the block output's BN + shortcut + ReLU
         for name, blk in self.blocks:
-            width, C4 = _block_widths(blk)
+            convs = self._convs[name]
+            n, C = len(convs), convs[-1].cout
             stride = blk.stride
             Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
             Min, Mout = B * Hc * Wc, B * Hn * Wn
-            rec = dict(name=name, x=x, Hin=Hc, Win=Wc, Hout=Hn, Wout=Wn, Cin=Cin, width=width, Cout=C4, stride=stride,
-                       Min=Min, Mout=Mout, has_ds=blk.downsample is not None, basic=isinstance(blk, BasicBlock))
-            if rec["basic"]:
-                # conv1 3x3 (stride) -> bn1 + ReLU -> conv2 3x3 -> bn2 + shortcut + ReLU (torchvision resnet.py:59-105)
-                y1 = ws.get(name + ".y1", (Mout, C4), BF16)
-                st1 = self._slab_take(2 * C4) if training else None
-                self._conv3x3(name + ".conv1", x, y1, B, Hc, Wc, stride, name + ".cols1", stats=st1)
-                a1 = ws.get(name + ".a1", (Mout, C4), BF16)
-                bnp1 = self._bn_act_fwd(y1, name + ".bn1", Mout, C4, training, st1, a1)
-                y2 = ws.get(name + ".y2", (Mout, C4), BF16)
-                st2 = self._slab_take(2 * C4) if training else None
-                self._conv3x3(name + ".conv2", a1, y2, B, Hn, Wn, 1, name + ".cols2", stats=st2)
-                out = ws.get(name + ".out", (Mout, C4), BF16)
-                m2 = ws.get(name + ".m2", (Mout, C4 // 8), torch.uint8) if training else None
-                bnp2 = self._block_output_fwd(rec, x, y2, st2, name + ".bn2", out, m2, B, training)
-                rec.update(y1=y1, bnp1=bnp1, a1=a1, y2=y2, bnp2=bnp2, out=out, m2=m2)
-                tape["blocks"].append(rec)
-                x, Hc, Wc, Cin = out, Hn, Wn, C4
-                continue
-            # conv1 1x1
-            y1 = ws.get(name + ".y1", (Min, width), BF16)
-            st1 = self._slab_take(2 * width) if training else None
-            gemm(x, self.W(name + ".conv1.weight").view(width, Cin), y1, Min, width, Cin, stats=st1)
-            a1 = ws.get(name + ".a1", (Min, width), BF16)
-            bnp1 = self._bn_act_fwd(y1, name + ".bn1", Min, width, training, st1, a1)
-            # conv2 3x3 (stride)
-            y2 = ws.get(name + ".y2", (Mout, width), BF16)
-            st2 = self._slab_take(2 * width) if training else None
-            rec["cols2"] = self._conv3x3(name + ".conv2", a1, y2, B, Hc, Wc, stride, name + ".cols2", stats=st2)
-            a2 = ws.get(name + ".a2", (Mout, width), BF16)
-            bnp2 = self._bn_act_fwd(y2, name + ".bn2", Mout, width, training, st2, a2)
-            # conv3 1x1
-            y3 = ws.get(name + ".y3", (Mout, C4), BF16)
-            st3 = self._slab_take(2 * C4) if training else None
-            gemm(a2, self.W(name + ".conv3.weight").view(C4, width), y3, Mout, C4, width, stats=st3)
-            out = ws.get(name + ".out", (Mout, C4), BF16)
+            rec = dict(name=name, x=x, Hin=Hc, Win=Wc, Hout=Hn, Wout=Wn, Cin=Cin, width=convs[0].cout, Cout=C,
+                       stride=stride, Min=Min, Mout=Mout, has_ds=blk.downsample is not None, basic=n == 2)
+            a, h, w = x, Hc, Wc
+            for i, conv in enumerate(convs, 1):
+                ho, wo = (h - 1) // conv.stride + 1, (w - 1) // conv.stride + 1
+                y = ws.get(f"{name}.y{i}", (B * ho * wo, conv.cout), BF16)
+                st = self._slab_take(2 * conv.cout) if training else None
+                rec[f"cols{i}"] = self._conv(conv, a, y, B, h, w, f"{name}.cols{i}", stats=st)
+                rec[f"y{i}"], rec[f"hw{i}"] = y, (h, w)  # hw: the conv's input grid
+                if i < n:
+                    a = ws.get(f"{name}.a{i}", y.shape, BF16)
+                    rec[f"a{i}"] = a
+                    rec[f"bnp{i}"] = self._bn_act_fwd(y, f"{name}.bn{i}", y.shape[0], conv.cout, training, st, a)
+                h, w = ho, wo
+            out = ws.get(name + ".out", (Mout, C), BF16)
             # backward needs only the SIGN of the block output's pre-activation: one bit per element instead of re-reading
             # the bf16 output twice (bn_bwd_reduce and bn_bwd_apply)
-            m3 = ws.get(name + ".m3", (Mout, C4 // 8), torch.uint8) if training else None
-            bnp3 = self._block_output_fwd(rec, x, y3, st3, name + ".bn3", out, m3, B, training)
-            rec.update(y1=y1, bnp1=bnp1, a1=a1, y2=y2, bnp2=bnp2, a2=a2, y3=y3, bnp3=bnp3, out=out, m3=m3)
+            m = ws.get(f"{name}.m{n}", (Mout, C // 8), torch.uint8) if training else None
+            rec[f"bnp{n}"] = self._block_output_fwd(rec, x, y, st, f"{name}.bn{n}", out, m, B, training)
+            rec.update({f"m{n}": m, "out": out})
             tape["blocks"].append(rec)
-            x, Hc, Wc, Cin = out, Hn, Wn, C4
+            x, Hc, Wc, Cin = out, Hn, Wn, C
         tape["feat"] = x
         tape["hw"] = (Hc, Wc)
         tape["C"] = Cin
@@ -564,36 +555,28 @@ class Engine:
         idx = ws.get("inf.stem.idx", (B * Hp * Wp, 64), torch.uint8)
         call("vtx_bn_relu_maxpool", y0.data_ptr(), ws.flat["bnp_eval:visual.cnn.bn1"].data_ptr(), x.data_ptr(),
              idx.data_ptr(), B, Ho, Wo, 64, s)
-        Hc, Wc, Cin = Hp, Wp, 64
-        # ---- residual blocks: each GEMM ends in its BN (+ shortcut) (+ ReLU), four per bottleneck, three per basic
-        # block with a downsample branch and two without; block outputs alternate between two buffers
+        Hc, Wc = Hp, Wp
+        # ---- residual blocks: each GEMM ends in its BN (+ shortcut) (+ ReLU): every conv but the last, the downsample,
+        # then the last conv with the shortcut; block outputs alternate between two buffers
         for bi, (name, blk) in enumerate(self.blocks):
-            width, C4 = _block_widths(blk)
-            basic = isinstance(blk, BasicBlock)
+            convs = self._convs[name]
+            n, C = len(convs), convs[-1].cout
             stride = blk.stride
             Hn, Wn = (Hc - 1) // stride + 1, (Wc - 1) // stride + 1
-            Min, Mout = B * Hc * Wc, B * Hn * Wn
-            if basic:
-                a1 = ws.get("inf.a1", (Mout, width), BF16)
-                self._conv3x3(name + ".conv1", x, a1, B, Hc, Wc, stride, "inf.cols1", act=1, **ss(name + ".bn1"))
-            else:
-                a1 = ws.get("inf.a1", (Min, width), BF16)
-                gemm(x, self.W(name + ".conv1.weight").view(width, Cin), a1, Min, width, Cin, act=1,
-                     **ss(name + ".bn1"))
-                a2 = ws.get("inf.a2", (Mout, width), BF16)
-                self._conv3x3(name + ".conv2", a1, a2, B, Hc, Wc, stride, "inf.cols2", act=1, **ss(name + ".bn2"))
+            Mout = B * Hn * Wn
+            a, h, w = x, Hc, Wc
+            for i, conv in enumerate(convs[:-1], 1):
+                ho, wo = (h - 1) // conv.stride + 1, (w - 1) // conv.stride + 1
+                y = ws.get(f"inf.a{i}", (B * ho * wo, conv.cout), BF16)
+                self._conv(conv, a, y, B, h, w, f"inf.cols{i}", act=1, **ss(f"{name}.bn{i}"))
+                a, h, w = y, ho, wo
             shortcut = x
             if blk.downsample is not None:
-                shortcut = ws.get("inf.shortcut", (Mout, C4), BF16)
+                shortcut = ws.get("inf.shortcut", (Mout, C), BF16)
                 self._downsample(name, x, shortcut, B, Hc, Wc, stride, "inf.xs", **ss(name + ".downsample.1"))
-            out = ws.get(f"inf.x{bi & 1}", (Mout, C4), BF16)
-            if basic:
-                self._conv3x3(name + ".conv2", a1, out, B, Hn, Wn, 1, "inf.cols2", residual=shortcut, act=1,
-                              **ss(name + ".bn2"))
-            else:
-                gemm(a2, self.W(name + ".conv3.weight").view(C4, width), out, Mout, C4, width, residual=shortcut,
-                     act=1, **ss(name + ".bn3"))
-            x, Hc, Wc, Cin = out, Hn, Wn, C4
+            out = ws.get(f"inf.x{bi & 1}", (Mout, C), BF16)
+            self._conv(convs[-1], a, out, B, h, w, f"inf.cols{n}", residual=shortcut, act=1, **ss(f"{name}.bn{n}"))
+            x, Hc, Wc = out, Hn, Wn
         return x, Hc, Wc
 
     # ------------------------------------------------------------------------------------------------ backbone bwd
@@ -629,12 +612,19 @@ class Engine:
                  y.data_ptr(), bnp.data_ptr(), dy.data_ptr(), y2.data_ptr(), bnp2.data_ptr(), dy2.data_ptr(),
                  _p(dz_out), M, C, mask_from_y, s)
 
-    def _wgrad3x3(self, dy, x, dwp, B, Hc, Wc, stride):
-        """Weight gradient of a 3x3 conv (stride) into its fp32 scratch dwp [C, 9 * Cin] (fp32 atomics): dy [Mout, C],
-        x [B*Hc*Wc, Cin], both read in place by implicit GEMMs."""
-        Mout, C = dy.shape
-        Cin = x.shape[1]
-        if _transposed_wgrad(Cin, C, stride):
+    def _conv_wgrad(self, conv, dy, x, cols, B, Hc, Wc):
+        """Weight gradient of main-branch conv `conv` from dy [Mout, C] and its input x [B*Hc*Wc, Cin]: a 1x1 conv's
+        straight into the gradient arena; a 3x3 conv's into its fp32 scratch _dwp [C, 9 * Cin] (fp32 atomics), from
+        the forward's im2col matrix `cols` when that route ran, else by an implicit GEMM over x."""
+        wname, k, stride, Cin, C = conv
+        Mout = dy.shape[0]
+        if k == 1:
+            self._wgrad(dy, x, self.G(wname + ".weight"), C, Cin, Mout)
+            return
+        dwp = self._dwp[wname].view(C, 9 * Cin)
+        if cols is not None:
+            self._wgrad(dy, cols, dwp, C, 9 * Cin, Mout)
+        elif _transposed_wgrad(Cin, C, stride):
             # wgrad in the [(tap, cin), cout] layout (vtx_conv_w_unpack_add_t folds it into OIHW)
             gemm(dy, x, dwp, 9 * Cin, C, Mout, atomic=True, lda=C, ldb=Cin, ldd=C, conv=(B, Hc, Wc, Cin), conv_mode=4,
                  out_f32=True)
@@ -644,12 +634,34 @@ class Engine:
             gemm(dy, x, dwp, C, 9 * Cin, Mout, atomic=True, split_k=sk, lda=C, ldb=Cin, conv=(B, Hc, Wc, Cin),
                  conv_mode=2, out_f32=True, conv_stride=stride)
 
+    def _conv_dgrad(self, conv, dy, dx, cols, B, Hc, Wc, **epi):
+        """Input gradient dx [B*Hc*Wc, Cin] of main-branch conv `conv` from dy [Mout, C], by the route _dgrad_route
+        picks.  `epi` (bnr, residual, residual_mask; None entries are dropped) goes to the epilogue of the GEMM that
+        writes dx; a route that cannot carry it raises."""
+        wname, k, stride, Cin, C = conv
+        epi = {key: v for key, v in epi.items() if v is not None}
+        route = _dgrad_route(conv, cols)
+        if route == "col2im" and epi or route == "parity" and set(epi) - {"bnr"}:
+            raise ValueError(f"the {route} dgrad of {wname} has no epilogue for {sorted(epi)}")
+        Mout, Min = dy.shape[0], dx.shape[0]
+        if route == "gemm":
+            gemm(dy, self.W(wname + ".weight").view(C, Cin), dx, Min, Cin, C, b_mn=1, **epi)
+        elif route == "implicit":
+            gemm(dy, self._packed[wname + ".weight#dgrad"], dx, Min, Cin, 9 * C, lda=C, conv=(B, Hc, Wc, C),
+                 conv_mode=1, **epi)
+        elif route == "parity":
+            self._dgrad3x3_s2(dy, wname, dx, B, Hc, Wc, **epi)
+        else:
+            dcols = self.ws.get("bwd.dcols", (Mout, 9 * Cin), BF16)
+            gemm(dy, self._packed[wname + ".weight"], dcols, Mout, 9 * Cin, C, b_mn=1)
+            call("vtx_col2im3x3", dcols.data_ptr(), dx.data_ptr(), B, Hc, Wc, Cin, stride, _stream())
+
     def _dgrad3x3_s2(self, dy, wname, dx, B, Hc, Wc, bnr=None):
         """Input gradient dx [B*Hc*Wc, Cin] of a stride-2 3x3 conv from dy [Mout, C] as four implicit GEMMs, one per
         parity class (ph, pw) of the input position: row 2i+ph of dx gathers dy rows i+a, a < 1+ph, through kernel rows
         ph+1-2a (same along w); each class writes its own strided sub-grid of dx, so every element is written exactly
-        once -- no per-tap gradient matrix, no col2im scatter.  bnr = (y, bnp, sums): the BN-backward sums of the BN
-        whose output gradient dx is, accumulated by the epilogues (ReLU mask recomputed from y)."""
+        once -- no per-tap gradient matrix, no col2im scatter.  bnr = (y, bnp, sums, None): the BN-backward sums of the
+        BN whose output gradient dx is, accumulated by the epilogues (ReLU mask recomputed from y)."""
         Mout, C = dy.shape
         Cin = dx.shape[1]
         Hn, Wn = (Hc - 1) // 2 + 1, (Wc - 1) // 2 + 1
@@ -660,7 +672,7 @@ class Engine:
                 if Hs <= 0 or Ws <= 0:
                     continue
                 voff = (ph * Wc + pw) * Cin * 2
-                epi = {} if bnr is None else dict(bnr=(bnr[0], bnr[1], bnr[2], None, bnr[0].data_ptr() + voff))
+                epi = {} if bnr is None else dict(bnr=(*bnr, bnr[0].data_ptr() + voff))
                 gemm(dy, self._packed[f"{wname}.weight#dgrad_s2_{ph}{pw}"], dx, Mout, Cin, th * tw * C, lda=C,
                      conv=(B, Hn, Wn, C), conv_mode=1, tap_grid=(th, tw, 0), d_ptr=dx.data_ptr() + voff,
                      out_view=(Hs, Ws, 2 * Cin, 2 * Wc * Cin, Hc * Wc * Cin), **epi)
@@ -710,88 +722,60 @@ class Engine:
         self._dwp_flat.zero_()
         stem_s2d = tape["stem"]["s2d"] is not None
         blocks = tape["blocks"]
-        sums3 = None  # bn3 sums of the current block when the GEMM that produced dOut already accumulated them
+        sums_out = None  # the current block's last-BN sums when the GEMM that produced dOut already accumulated them
         for bi in range(len(blocks) - 1, -1, -1):
             rec = blocks[bi]
-            name, width, Cin, stride = rec["name"], rec["width"], rec["Cin"], rec["stride"]
+            name, Cin = rec["name"], rec["Cin"]
             layer = name.split(".")[2]
             if prev_layer is not None and layer != prev_layer:
                 self._run_jobs("unpack:" + prev_layer, lambda: self._unpack_rows(prev_layer, stem_s2d))
                 if bucket_cb is not None:
                     bucket_cb(prev_layer)
             prev_layer = layer
-            Min, Mout, C4 = rec["Min"], rec["Mout"], rec["Cout"]
-            Hc, Wc, Hn, Wn = rec["Hin"], rec["Win"], rec["Hout"], rec["Wout"]
-            if rec["basic"]:
-                dOut, sums3 = self._basic_block_bwd(rec, blocks[bi - 1] if bi > 0 else None, dOut, sums3,
-                                                    ws.get(f"bwd.dx{scratch_i & 1}", (Min, Cin), BF16), B)
-                scratch_i += 1
-                continue
-            # ---- block output: ReLU mask + bn3 (+ downsample BN) backward
-            dy3 = ws.get("bwd.dy3", (Mout, C4), BF16)
+            convs = self._convs[name]
+            n, Min, Mout, C = len(convs), rec["Min"], rec["Mout"], rec["Cout"]
+            # ---- block output: ReLU mask + the last BN (+ downsample BN) backward
+            dy = ws.get(f"bwd.dy{n}", (Mout, C), BF16)
+            m, y, bnp, bn_name = rec[f"m{n}"], rec[f"y{n}"], rec[f"bnp{n}"], f"{name}.bn{n}"
             if rec["has_ds"]:
-                dyd = ws.get("bwd.dyd", (Mout, C4), BF16)
-                self._bn_bwd(dOut, rec["m3"], rec["y3"], rec["bnp3"], name + ".bn3", Mout, C4, dy3,
+                dyd = ws.get("bwd.dyd", (Mout, C), BF16)
+                self._bn_bwd(dOut, m, y, bnp, bn_name, Mout, C, dy,
                              two=(rec["yd"], rec["bnpd"], name + ".downsample.1", dyd))
-                dz = None
             else:
                 # the shortcut gradient dz = dOut * [block output > 0] is never written: conv1's dgrad epilogue adds
                 # dOut under the same bit mask (VtxGemm.residual_mask)
-                dz = None
-                self._bn_bwd(dOut, rec["m3"], rec["y3"], rec["bnp3"], name + ".bn3", Mout, C4, dy3, sums=sums3)
-            sums3 = None
-            # ---- conv3 (1x1): wgrad + dgrad; the dgrad epilogue accumulates bn2's backward sums (ReLU mask from y2)
-            self._wgrad(dy3, rec["a2"], self.G(name + ".conv3.weight"), C4, width, Mout)
-            da2 = ws.get("bwd.da2", (Mout, width), BF16)
-            sums2 = self._slab_take(2 * width)
-            gemm(dy3, self.W(name + ".conv3.weight").view(C4, width), da2, Mout, width, C4, b_mn=1,
-                 bnr=(rec["y2"], rec["bnp2"], sums2, None))
-            # ---- bn2 + ReLU backward
-            dy2 = ws.get("bwd.dy2", (Mout, width), BF16)
-            self._bn_bwd(da2, None, rec["y2"], rec["bnp2"], name + ".bn2", Mout, width, dy2, mask_from_y=1, sums=sums2)
-            # ---- conv2 (3x3): wgrad + dgrad
-            dwp = self._dwp[name + ".conv2"].view(width, 9 * width)
-            da1 = ws.get("bwd.da1", (Min, width), BF16)
-            sums1 = None
-            if rec["cols2"] is None:
-                self._wgrad3x3(dy2, rec["a1"], dwp, B, Hc, Wc, stride)
-                if stride in (1, 2):
-                    sums1 = self._slab_take(2 * width)  # bn1's backward sums, accumulated by the conv2-dgrad epilogue(s)
-                if stride == 1:
-                    gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Min, width, 9 * width, lda=width,
-                         conv=(B, Hc, Wc, width), conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
-                elif stride == 2:
-                    self._dgrad3x3_s2(dy2, name + ".conv2", da1, B, Hc, Wc, bnr=(rec["y1"], rec["bnp1"], sums1))
-                else:  # other strides: per-tap gradients by a plain GEMM, scattered back by col2im
-                    dcols = ws.get("bwd.dcols", (Mout, 9 * width), BF16)
-                    gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * width, width, b_mn=1)
-                    call("vtx_col2im3x3", dcols.data_ptr(), da1.data_ptr(), B, Hc, Wc, width, stride, s)
-            else:
-                self._wgrad(dy2, rec["cols2"], dwp, width, 9 * width, Mout)
-                dcols = ws.get("bwd.dcols", (Mout, 9 * width), BF16)
-                gemm(dy2, self._packed[name + ".conv2.weight"], dcols, Mout, 9 * width, width, b_mn=1)
-                call("vtx_col2im3x3", dcols.data_ptr(), da1.data_ptr(), B, Hc, Wc, width, stride, s)
-            # ---- bn1 + ReLU backward
-            dy1 = ws.get("bwd.dy1", (Min, width), BF16)
-            self._bn_bwd(da1, None, rec["y1"], rec["bnp1"], name + ".bn1", Min, width, dy1, mask_from_y=1, sums=sums1)
-            # ---- conv1 (1x1): wgrad + dgrad (+ shortcut gradient)
-            self._wgrad(dy1, rec["x"], self.G(name + ".conv1.weight"), width, Cin, Min)
+                self._bn_bwd(dOut, m, y, bnp, bn_name, Mout, C, dy, sums=sums_out)
+            sums_out = None
+            # ---- conv n .. conv2: wgrad + dgrad, whose epilogue accumulates the backward sums of the BN before it
+            # (ReLU mask recomputed from its y) wherever the route allows; then that BN's backward
+            for i in range(n, 1, -1):
+                conv, cols, (h, w) = convs[i - 1], rec[f"cols{i}"], rec[f"hw{i}"]
+                y, bnp = rec[f"y{i - 1}"], rec[f"bnp{i - 1}"]
+                self._conv_wgrad(conv, dy, rec[f"a{i - 1}"], cols, B, h, w)
+                da = ws.get(f"bwd.da{i - 1}", y.shape, BF16)
+                sums = self._slab_take(2 * conv.cin) if _dgrad_route(conv, cols) != "col2im" else None
+                self._conv_dgrad(conv, dy, da, cols, B, h, w, bnr=None if sums is None else (y, bnp, sums, None))
+                dy = ws.get(f"bwd.dy{i - 1}", y.shape, BF16)
+                self._bn_bwd(da, None, y, bnp, f"{name}.bn{i - 1}", y.shape[0], conv.cin, dy, mask_from_y=1, sums=sums)
+            # ---- conv1: wgrad + dgrad (+ shortcut gradient)
+            conv, cols, (h, w) = convs[0], rec["cols1"], rec["hw1"]
+            self._conv_wgrad(conv, dy, rec["x"], cols, B, h, w)
             dx = ws.get(f"bwd.dx{scratch_i & 1}", (Min, Cin), BF16)
             scratch_i += 1
-            w1 = self.W(name + ".conv1.weight").view(width, Cin)
             if rec["has_ds"]:
                 self._downsample_wgrad(rec, dyd, B)
-                gemm(dy1, w1, dx, Min, Cin, width, b_mn=1)
+                self._conv_dgrad(conv, dy, dx, cols, B, h, w)
                 self._downsample_dgrad_add(rec, dyd, dx, B)
             else:
-                # dx is the output gradient of the previous block: when that block has a single-branch bn3, its backward
-                # sums (ReLU bit mask m3 of THAT block) are accumulated here, over the staged dx tiles
+                # dx is the output gradient of the previous block: when that block has a single-branch last BN, its
+                # backward sums (ReLU bit mask of THAT block) are accumulated here, over the staged dx tiles
                 prev = blocks[bi - 1] if bi > 0 else None
-                bnr3 = None
+                bnr = None
                 if prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
-                    sums3 = self._slab_take(2 * Cin)
-                    bnr3 = (prev["y3"], prev["bnp3"], sums3, prev["m3"])
-                gemm(dy1, w1, dx, Min, Cin, width, b_mn=1, residual=dOut, residual_mask=rec["m3"], bnr=bnr3)
+                    p = len(self._convs[prev["name"]])
+                    sums_out = self._slab_take(2 * Cin)
+                    bnr = (prev[f"y{p}"], prev[f"bnp{p}"], sums_out, prev[f"m{p}"])
+                self._conv_dgrad(conv, dy, dx, cols, B, h, w, residual=dOut, residual_mask=rec[f"m{n}"], bnr=bnr)
             dOut = dx
         # ---- stem: maxpool bwd -> ReLU/BN bwd -> wgrad
         st = tape["stem"]
@@ -809,53 +793,6 @@ class Engine:
             self._wgrad(dy0, st["cols"], dwp0, 64, 160, M0)
         # layer1's 3x3 weight gradients + the stem's, in one launch (the 'rest' all-reduce bucket follows)
         self._run_jobs("unpack:rest:" + ("s2d" if stem_s2d else "cols"), lambda: self._unpack_rows("rest", stem_s2d))
-
-    def _basic_block_bwd(self, rec, prev, dOut, sums2, dx, B):
-        """Backward of one basic block from its output gradient dOut into dx [Min, Cin], its parameter gradients
-        accumulated; `sums2`: bn2's backward sums when the GEMM that produced dOut already accumulated them.  Returns
-        (dx, the previous block's bn2 sums when this block's conv1 dgrad accumulated them, else None)."""
-        ws = self.ws
-        name, Cin, C, stride = rec["name"], rec["Cin"], rec["Cout"], rec["stride"]
-        Min, Mout, Hn, Wn = rec["Min"], rec["Mout"], rec["Hout"], rec["Wout"]
-        # ---- block output: ReLU mask + bn2 (+ downsample BN) backward
-        dy2 = ws.get("bwd.dy2", (Mout, C), BF16)
-        dyd = None
-        if rec["has_ds"]:
-            dyd = ws.get("bwd.dyd", (Mout, C), BF16)
-            self._bn_bwd(dOut, rec["m2"], rec["y2"], rec["bnp2"], name + ".bn2", Mout, C, dy2,
-                         two=(rec["yd"], rec["bnpd"], name + ".downsample.1", dyd))
-        else:
-            self._bn_bwd(dOut, rec["m2"], rec["y2"], rec["bnp2"], name + ".bn2", Mout, C, dy2, sums=sums2)
-        # ---- conv2 (3x3, stride 1): wgrad + dgrad; the dgrad epilogue accumulates bn1's sums (ReLU mask from y1)
-        self._wgrad3x3(dy2, rec["a1"], self._dwp[name + ".conv2"].view(C, 9 * C), B, Hn, Wn, 1)
-        da1 = ws.get("bwd.da1", (Mout, C), BF16)
-        sums1 = self._slab_take(2 * C)
-        gemm(dy2, self._packed[name + ".conv2.weight#dgrad"], da1, Mout, C, 9 * C, lda=C, conv=(B, Hn, Wn, C),
-             conv_mode=1, bnr=(rec["y1"], rec["bnp1"], sums1, None))
-        dy1 = ws.get("bwd.dy1", (Mout, C), BF16)
-        self._bn_bwd(da1, None, rec["y1"], rec["bnp1"], name + ".bn1", Mout, C, dy1, mask_from_y=1, sums=sums1)
-        # ---- conv1 (3x3, stride): wgrad + dgrad (+ shortcut gradient)
-        Hc, Wc = rec["Hin"], rec["Win"]
-        self._wgrad3x3(dy1, rec["x"], self._dwp[name + ".conv1"].view(C, 9 * Cin), B, Hc, Wc, stride)
-        if rec["has_ds"]:
-            self._downsample_wgrad(rec, dyd, B)
-            if stride == 2:
-                self._dgrad3x3_s2(dy1, name + ".conv1", dx, B, Hc, Wc)
-            else:
-                gemm(dy1, self._packed[name + ".conv1.weight#dgrad"], dx, Min, Cin, 9 * C, lda=C, conv=(B, Hc, Wc, C),
-                     conv_mode=1)
-            self._downsample_dgrad_add(rec, dyd, dx, B)
-            return dx, None
-        # identity block: the shortcut gradient dOut * [block output > 0] is never written -- conv1's dgrad epilogue
-        # adds dOut under the block's bit mask; dx is the output gradient of the previous block, whose bn2 sums (under
-        # THAT block's bit mask) the same epilogue accumulates when the previous block has a single-branch bn2
-        bnr, sums_prev = None, None
-        if prev is not None and not prev["has_ds"] and Cin % 32 == 0 and Min >= self.fuse_bn3_min_rows:
-            sums_prev = self._slab_take(2 * Cin)
-            bnr = (prev["y2"], prev["bnp2"], sums_prev, prev["m2"])
-        gemm(dy1, self._packed[name + ".conv1.weight#dgrad"], dx, Min, Cin, 9 * C, lda=C, conv=(B, Hc, Wc, C),
-             conv_mode=1, residual=dOut, residual_mask=rec["m2"], bnr=bnr)
-        return dx, sums_prev
 
     # ------------------------------------------------------------------------------------------------ head
     def _head_modules(self, direction):
